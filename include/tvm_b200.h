@@ -259,6 +259,32 @@ int tvm_main_table_from_aet(tvm_ctx *ctx, const tvm_aet *aet, uint64_t num_rows,
 int tvm_prove_aet(tvm_ctx *ctx, const tvm_params *params, const tvm_claim *claim, uint64_t padded_height, const tvm_aet *aet,
                   const uint64_t *main_rand, const uint64_t *aux_rand, const uint64_t *randomizer_column, const uint64_t *quot_rand,
                   uint64_t *proof_out, size_t *proof_len);
+/* ---- Seeded proving: the prover's randomness drawn on the device from ONE 32-byte seed, exactly as Prover::prove draws it
+ *      from its `randomness_seed` (stark.rs:192, 293-328): every array comes from its own
+ *      StdRng::from_seed(offset_rng_seed(seed, k)) stream (master_table.rs:630-662; StdRng = ChaCha12, each B-field element one
+ *      sample of rand's `random_range(0..=p-1)`, each X-field element three):
+ *        main_rand          [379][h]     k = column                     (trace_randomizer_for_column, master_table.rs:423-434)
+ *        aux_rand           [91][h][3]   k = 379 + column               (offset_rng_seed(offset_rng_seed(seed, 379), column))
+ *        randomizer_column  [n][3]       k = 379 + 91                   (auxiliary column 90, master_table.rs:1016-1023)
+ *        quot_rand          [(h+1)*5][3] k = 379 + 91 + 1               (quotient-segment randomizer, stark.rs:1316-1322)
+ *      h, n and the quotient coefficient count as tvm_derive_domains reports them for `params` and `padded_height`.
+ *      WARNING (as the reference's Prover::set_randomness_seed_which_may_break_zero_knowledge): the proof is zero-knowledge
+ *      only if the seed comes from a cryptographically secure RNG that the verifier can neither predict nor influence (what
+ *      Prover::new does with `random()`).  A fixed or reused seed breaks zero knowledge.  The library never draws entropy
+ *      itself: it stays a deterministic function of its inputs, and a NULL seed is TVM_ERR_INVALID_ARG.
+ *
+ *      tvm_prover_randomness: kernel-level entry point; the four arrays (canonical) into host or device memory, any of them
+ *      may be NULL.
+ *      tvm_prove_aet_seeded / tvm_prove_tables_seeded: the proof words tvm_prove_aet / tvm_prove_tables give when handed the
+ *      arrays tvm_prover_randomness returns for the same seed.  The randomness is generated in device memory and never
+ *      crosses PCIe.  With tvm_ctx_set_comm every rank is handed the same seed and derives the identical randomness itself. */
+int tvm_prover_randomness(tvm_ctx *ctx, const tvm_params *params, uint64_t padded_height, const uint8_t seed[32], uint64_t *main_rand_out,
+                          uint64_t *aux_rand_out, uint64_t *randomizer_column_out, uint64_t *quot_rand_out);
+int tvm_prove_aet_seeded(tvm_ctx *ctx, const tvm_params *params, const tvm_claim *claim, uint64_t padded_height, const tvm_aet *aet,
+                         const uint8_t seed[32], uint64_t *proof_out, size_t *proof_len);
+int tvm_prove_tables_seeded(tvm_ctx *ctx, const tvm_params *params, const tvm_claim *claim, uint64_t padded_height,
+                            const uint64_t *main_table, int fill_derived_main_columns, const uint8_t seed[32], uint64_t *proof_out,
+                            size_t *proof_len);
 /* Bezout coefficient polynomials of rp = prod (x - roots[i]) and its formal derivative (ram.rs:162-214), kernel-level entry
  * point: `roots` m distinct canonical elements; a_out, b_out [m] canonical coefficients, lowest first. */
 int tvm_bezout_coefficients(tvm_ctx *ctx, const uint64_t *roots, uint64_t m, uint64_t *a_out, uint64_t *b_out);

@@ -140,6 +140,21 @@ static bool claim_ok(const tvm_claim *c) {
   return true;
 }
 
+// the prover's randomness for `seed` in device memory of `mem` (canonical; main, aux, column 90, quotient segments)
+struct SeededRandomness {
+  const u64 *main_rand, *aux_rand, *randomizer_column, *quot_rand;
+  size_t n, h, nq;   // trace length, trace randomizers, quotient randomizer coefficients
+};
+static SeededRandomness seeded_randomness(Ctx &c, DevMem &mem, const StarkParams &sp, uint64_t padded_height, const uint8_t *seed) {
+  StarkDerived d{};
+  if (int rc = stark_derive(sp, padded_height, d)) throw ApiError{rc, "parameter derivation failed"};
+  const ProverRandomnessLayout L = prover_randomness_layout(d.trace_len, d.num_trace_randomizers, d.num_quotient_randomizer_coefficients);
+  u64 *d_r = mem.words(L.total);
+  prover_randomness_run(c, seed, d.trace_len, d.num_trace_randomizers, d.num_quotient_randomizer_coefficients, d_r);
+  return {d_r + L.main, d_r + L.aux, d_r + L.randomizer_column, d_r + L.quot, d.trace_len, d.num_trace_randomizers,
+          d.num_quotient_randomizer_coefficients};
+}
+
 extern "C" {
 
 int tvm_device_count(void) {
@@ -555,6 +570,65 @@ int tvm_prove_aet(tvm_ctx *ctx, const tvm_params *params, const tvm_claim *claim
   DeviceTables dt{(const u64 *)aux_rand, (const u64 *)randomizer_column, true, aet};
   stark_prove(*c__, StarkParams{params->security_level, params->log2_ldt_expansion_factor, params->ldt_choice, params->soundness}, cv, padded_height,
               nullptr, (const u64 *)main_rand, nullptr, nullptr, (const u64 *)quot_rand, proof, &ctx->timings, &dt);
+  size_t cap = *proof_len;
+  *proof_len = proof.size();
+  if (!proof_out || cap < proof.size()) throw ApiError{TVM_ERR_INVALID_ARG, "proof buffer too small"};
+  memcpy(proof_out, proof.data(), proof.size() * 8);
+  TVM_API_END
+}
+
+int tvm_prover_randomness(tvm_ctx *ctx, const tvm_params *params, uint64_t padded_height, const uint8_t seed[32], uint64_t *main_rand_out,
+                          uint64_t *aux_rand_out, uint64_t *randomizer_column_out, uint64_t *quot_rand_out) {
+  if (!ctx || !params || !seed || params->ldt_choice > 2) return TVM_ERR_INVALID_ARG;
+  TVM_API_BEGIN(ctx)
+  Ctx &c = *c__;
+  const StarkParams sp{params->security_level, params->log2_ldt_expansion_factor, params->ldt_choice, params->soundness};
+  DevMem mem(c);
+  const SeededRandomness r = seeded_randomness(c, mem, sp, padded_height, seed);
+  if (main_rand_out) TVM_CUDA(cudaMemcpyAsync(main_rand_out, r.main_rand, TVM_NUM_MAIN_COLUMNS * r.h * 8, cudaMemcpyDefault, c.stream));
+  if (aux_rand_out) TVM_CUDA(cudaMemcpyAsync(aux_rand_out, r.aux_rand, TVM_NUM_AUX_COLUMNS * r.h * 3 * 8, cudaMemcpyDefault, c.stream));
+  if (randomizer_column_out) TVM_CUDA(cudaMemcpyAsync(randomizer_column_out, r.randomizer_column, r.n * 3 * 8, cudaMemcpyDefault, c.stream));
+  if (quot_rand_out) TVM_CUDA(cudaMemcpyAsync(quot_rand_out, r.quot_rand, r.nq * 3 * 8, cudaMemcpyDefault, c.stream));
+  TVM_CUDA(cudaStreamSynchronize(c.stream));
+  TVM_API_END
+}
+
+int tvm_prove_aet_seeded(tvm_ctx *ctx, const tvm_params *params, const tvm_claim *claim, uint64_t padded_height, const tvm_aet *aet,
+                         const uint8_t seed[32], uint64_t *proof_out, size_t *proof_len) {
+  if (!ctx || !params || !claim || !aet || !seed || !proof_len) return TVM_ERR_INVALID_ARG;
+  if (params->ldt_choice > 2 || !claim_ok(claim)) return TVM_ERR_INVALID_ARG;
+  TVM_API_BEGIN(ctx)
+  const StarkParams sp{params->security_level, params->log2_ldt_expansion_factor, params->ldt_choice, params->soundness};
+  ClaimView cv{claim->program_digest, claim->version, claim->input, claim->num_input, claim->output, claim->num_output};
+  std::vector<u64> proof;
+  {
+    DevMem mem(*c__);
+    const SeededRandomness r = seeded_randomness(*c__, mem, sp, padded_height, seed);
+    DeviceTables dt{r.aux_rand, r.randomizer_column, true, aet};
+    stark_prove(*c__, sp, cv, padded_height, nullptr, r.main_rand, nullptr, nullptr, r.quot_rand, proof, &ctx->timings, &dt);
+  }
+  size_t cap = *proof_len;
+  *proof_len = proof.size();
+  if (!proof_out || cap < proof.size()) throw ApiError{TVM_ERR_INVALID_ARG, "proof buffer too small"};
+  memcpy(proof_out, proof.data(), proof.size() * 8);
+  TVM_API_END
+}
+
+int tvm_prove_tables_seeded(tvm_ctx *ctx, const tvm_params *params, const tvm_claim *claim, uint64_t padded_height,
+                            const uint64_t *main_table, int fill_derived_main_columns, const uint8_t seed[32], uint64_t *proof_out,
+                            size_t *proof_len) {
+  if (!ctx || !params || !claim || !main_table || !seed || !proof_len) return TVM_ERR_INVALID_ARG;
+  if (params->ldt_choice > 2 || !claim_ok(claim)) return TVM_ERR_INVALID_ARG;
+  TVM_API_BEGIN(ctx)
+  const StarkParams sp{params->security_level, params->log2_ldt_expansion_factor, params->ldt_choice, params->soundness};
+  ClaimView cv{claim->program_digest, claim->version, claim->input, claim->num_input, claim->output, claim->num_output};
+  std::vector<u64> proof;
+  {
+    DevMem mem(*c__);
+    const SeededRandomness r = seeded_randomness(*c__, mem, sp, padded_height, seed);
+    DeviceTables dt{r.aux_rand, r.randomizer_column, fill_derived_main_columns != 0};
+    stark_prove(*c__, sp, cv, padded_height, (const u64 *)main_table, r.main_rand, nullptr, nullptr, r.quot_rand, proof, &ctx->timings, &dt);
+  }
   size_t cap = *proof_len;
   *proof_len = proof.size();
   if (!proof_out || cap < proof.size()) throw ApiError{TVM_ERR_INVALID_ARG, "proof buffer too small"};

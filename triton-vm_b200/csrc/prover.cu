@@ -545,7 +545,7 @@ void stark_prove(Ctx &c, const StarkParams &sp, const ClaimView &claim, size_t p
   const size_t nqr = d.num_quotient_randomizer_coefficients;
   u64 *d_qr_in = mem.words(3 * nqr);
   u64 *d_qr = mem.words(3 * nqr);
-  TVM_CUDA(cudaMemcpyAsync(d_qr_in, h_quot_rand, 3 * nqr * 8, cudaMemcpyHostToDevice, c.stream));
+  TVM_CUDA(cudaMemcpyAsync(d_qr_in, h_quot_rand, 3 * nqr * 8, cudaMemcpyDefault, c.stream));   // host, or device (seeded proves)
   to_mont_run(c, d_qr_in, 3 * nqr);
   deinterleave3_run(c, d_qr_in, d_qr, nqr, 1);
   u64 *d_seg_coef = mem.words(15 * seg_len);

@@ -69,6 +69,13 @@ void stark_prove(Ctx &c, const StarkParams &sp, const ClaimView &claim, size_t p
 void main_fill_run(Ctx &c, struct DevMem &mem, const tvm_aet &aet, size_t n, u64 *d_table, uint64_t *lengths9);
 void bezout_run(Ctx &c, struct DevMem &mem, const u64 *d_roots_mont, size_t m, u64 *d_a, u64 *d_b);
 
+// ---- prover_randomness.cu: the prover's four randomness arrays from its 32-byte seed, CANONICAL, concatenated ----
+struct ProverRandomnessLayout {   // word offsets into the concatenation, and its length
+  size_t main, aux, randomizer_column, quot, total;   // [379][h], [91][h][3], [n][3], [nq][3]
+};
+ProverRandomnessLayout prover_randomness_layout(size_t n, size_t h, size_t nq);
+void prover_randomness_run(Ctx &c, const uint8_t seed[32], size_t n, size_t h, size_t nq, u64 *d_out);
+
 // ---- stark_kernels.cu ----
 struct SegmentArgs {
   const u64 *quot; size_t quot_stride;

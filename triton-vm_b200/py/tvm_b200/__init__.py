@@ -165,6 +165,11 @@ _SIGNATURES = {
     "tvm_prove_aet": (ctypes.c_int, [_vp, ctypes.POINTER(Params), ctypes.POINTER(ClaimStruct), ctypes.c_uint64, ctypes.POINTER(AetStruct),
                                      _u64p, _u64p, _u64p, _u64p, _u64p, ctypes.POINTER(ctypes.c_size_t)]),
     "tvm_bezout_coefficients": (ctypes.c_int, [_vp, _u64p, ctypes.c_uint64, _u64p, _u64p]),
+    "tvm_prover_randomness": (ctypes.c_int, [_vp, ctypes.POINTER(Params), ctypes.c_uint64, ctypes.c_char_p, _u64p, _u64p, _u64p, _u64p]),
+    "tvm_prove_aet_seeded": (ctypes.c_int, [_vp, ctypes.POINTER(Params), ctypes.POINTER(ClaimStruct), ctypes.c_uint64,
+                                            ctypes.POINTER(AetStruct), ctypes.c_char_p, _u64p, ctypes.POINTER(ctypes.c_size_t)]),
+    "tvm_prove_tables_seeded": (ctypes.c_int, [_vp, ctypes.POINTER(Params), ctypes.POINTER(ClaimStruct), ctypes.c_uint64, _u64p,
+                                               ctypes.c_int, ctypes.c_char_p, _u64p, ctypes.POINTER(ctypes.c_size_t)]),
     "tvm_prove_transcript": (ctypes.c_int, [_vp, ctypes.POINTER(Params), ctypes.POINTER(ClaimStruct), ctypes.c_uint64, _u64p, _u64p,
                                             AUX_CALLBACK, _vp, _u64p, ctypes.c_void_p]),
     "tvm_stir_prove": (ctypes.c_int, [_vp, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, _u64p, _u64p,
@@ -620,6 +625,84 @@ class Backend:
         rc = self._l.tvm_prove_aet(self._h, ctypes.byref(p), ctypes.byref(cs), ph, ctypes.byref(s), mrp, arp, rcp, qrp,
                                    buf.ctypes.data_as(_u64p), ctypes.byref(cap))
         del keep
+        self._chk(rc)
+        return buf[:cap.value].copy()
+
+    @staticmethod
+    def _seed(seed):
+        """32 seed bytes (None passes NULL, which the library rejects)"""
+        if seed is None:
+            return None
+        seed = bytes(seed)
+        assert len(seed) == 32, "the prover's randomness seed is 32 bytes"
+        return seed
+
+    @staticmethod
+    def _claim(claim):
+        digest, inp, out = claim[0], claim[1], claim[2]
+        version = claim[3] if len(claim) > 3 else 6
+        ia, iap = _np_u64(np.array(list(inp), dtype=np.uint64))
+        oa, oap = _np_u64(np.array(list(out), dtype=np.uint64))
+        return ClaimStruct((ctypes.c_uint64 * 5)(*[int(v) for v in digest]), version, iap, ia.size, oap, oa.size), (ia, oa)
+
+    def prover_randomness(self, seed, padded_height, security_level=160, log2_expansion=2, ldt_choice=LDT_AUTO, conjectured=False,
+                          out=None):
+        """tvm_prover_randomness: the prover's randomness drawn on the device from its 32-byte seed, as Prover::prove draws it
+        -> (main_rand [379, h], aux_rand [91, h, 3], randomizer_column [n, 3], quot_rand [(h+1)*5, 3]), canonical.
+        `out`: optional 4-tuple of destination arrays (numpy or contiguous torch tensors, host or CUDA; None skips one);
+        by default four new numpy arrays."""
+        dom = derive_domains(security_level, log2_expansion, padded_height, ldt_choice, conjectured)
+        h, n, nq = dom["num_trace_randomizers"], dom["trace_len"], dom["num_quotient_randomizer_coefficients"]
+        shapes = [(NUM_MAIN_COLUMNS, h), (NUM_AUX_COLUMNS, h, 3), (n, 3), (nq, 3)]
+        if out is None:
+            out = tuple(np.empty(s, dtype=np.uint64) for s in shapes)
+        ptrs = []
+        for o, s in zip(out, shapes):
+            if o is None:
+                ptrs.append(None)
+                continue
+            _, op, shape = _u64_arg(o)
+            assert int(np.prod(shape)) == int(np.prod(s)), (shape, s)
+            if isinstance(o, np.ndarray):
+                assert o.flags.c_contiguous and o.dtype == np.uint64
+            ptrs.append(op)
+        p = Params(security_level, log2_expansion, ldt_choice, int(conjectured))
+        self._chk(self._l.tvm_prover_randomness(self._h, ctypes.byref(p), padded_height, self._seed(seed), *ptrs))
+        return out
+
+    def prove_aet_seeded(self, claim, aet, seed, padded_height, security_level=160, log2_expansion=2, ldt_choice=LDT_AUTO,
+                         conjectured=False):
+        """tvm_prove_aet_seeded: Stark::prove from the AlgebraicExecutionTrace and the prover's 32-byte randomness seed alone —
+        the proof Prover::prove gives with that seed.  The seed must come from a CSPRNG the verifier cannot predict."""
+        s, keep = aet_struct(aet)
+        ph = int(padded_height)
+        dom = derive_domains(security_level, log2_expansion, ph, ldt_choice, conjectured)
+        cs, keep_claim = self._claim(claim)
+        p = Params(security_level, log2_expansion, ldt_choice, int(conjectured))
+        est = _proof_capacity(dom)
+        buf = np.empty(est, dtype=np.uint64)
+        cap = ctypes.c_size_t(est)
+        rc = self._l.tvm_prove_aet_seeded(self._h, ctypes.byref(p), ctypes.byref(cs), ph, ctypes.byref(s), self._seed(seed),
+                                          buf.ctypes.data_as(_u64p), ctypes.byref(cap))
+        del keep, keep_claim
+        self._chk(rc)
+        return buf[:cap.value].copy()
+
+    def prove_tables_seeded(self, claim, main_table, seed, security_level=160, log2_expansion=2, padded_height=None, ldt_choice=LDT_AUTO,
+                            conjectured=False, fill_derived_main_columns=True):
+        """tvm_prove_tables_seeded: as prove_tables, with the randomness drawn on the device from the prover's 32-byte seed."""
+        mt, mtp, mt_shape = _u64_arg(main_table)
+        ph = padded_height or mt_shape[1]
+        dom = derive_domains(security_level, log2_expansion, ph, ldt_choice, conjectured)
+        assert mt_shape == (379, dom["trace_len"]), mt_shape
+        cs, keep_claim = self._claim(claim)
+        p = Params(security_level, log2_expansion, ldt_choice, int(conjectured))
+        est = _proof_capacity(dom)
+        buf = np.empty(est, dtype=np.uint64)
+        cap = ctypes.c_size_t(est)
+        rc = self._l.tvm_prove_tables_seeded(self._h, ctypes.byref(p), ctypes.byref(cs), ph, mtp, int(bool(fill_derived_main_columns)),
+                                             self._seed(seed), buf.ctypes.data_as(_u64p), ctypes.byref(cap))
+        del keep_claim
         self._chk(rc)
         return buf[:cap.value].copy()
 
