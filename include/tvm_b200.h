@@ -304,6 +304,38 @@ int tvm_stir_prove(tvm_ctx *ctx, uint32_t security_level, uint32_t soundness, ui
 int tvm_stir_verify(uint32_t security_level, uint32_t soundness, uint32_t log2_initial_expansion_factor, uint32_t log2_high_degree_bound,
                     const uint64_t *proof, size_t proof_len, uint32_t *indices_out, uint64_t *values_out, size_t *num_indices,
                     char *failure, size_t failure_capacity);
+/* ---- FRI as a stand-alone low-degree test: Fri::prove / Fri::verify (low_degree_test/fri.rs:212-366, 393-735, 754-789) of the
+ *      sealed `LowDegreeTest` trait for ARBITRARY FriParameters (fri.rs:799-845): the prover Stark::default() uses below padded
+ *      height 2^16 and LdtChoice::Fri everywhere, for hosts that keep Prover::prove's orchestration and for the restated
+ *      property tests of the reference (fri.rs:989-1425).  The initial domain has 2^(log2_high_degree_bound +
+ *      log2_initial_expansion_factor) points and offset BFieldElement::generator() (fri.rs:829).  The whole prove and
+ *      tvm_verify run the same prover and verifier.
+ *      Parameter errors are LdtParameterError's (fri.rs:800-829): TVM_ERR_LDT_PARAMS for log2_initial_expansion_factor == 0
+ *      (TooSmallInitialExpansionFactor), >= 32 (TooBigInitialExpansionFactor) or an initial domain beyond 2^32 points
+ *      (InitialDomainTooBig); the variant is named in tvm_last_error / `failure`. --- */
+typedef struct tvm_fri_info {
+  uint64_t domain_len, domain_offset, expansion_factor, max_degree;   /* domain_offset canonical; max_degree = Fri::max_degree */
+  uint64_t num_collinearity_checks, num_rounds, last_round_max_degree;
+} tvm_fri_info;
+/* host code, no GPU: FriParameters::try_into_fri and Fri::{max_degree, num_rounds, last_round_max_degree} (fri.rs:799-924) */
+int tvm_fri_derive(uint32_t security_level, uint32_t soundness, uint32_t log2_initial_expansion_factor, uint32_t log2_high_degree_bound,
+                   tvm_fri_info *out);
+/*      codeword     [codeword_len][3] canonical X-field evaluations on the initial domain (host or device memory);
+ *                   codeword_len != domain length is TVM_ERR_INVALID_ARG, "InitialCodewordMismatch { domain_len, codeword_len }"
+ *                   (LdtProvingError, fri.rs:323-330).  Initial domains beyond 2^26 points are TVM_ERR_DOMAIN.
+ *      proof_out    the encoded proof stream of the FRI items alone (Proof.0 layout; same capacity protocol as tvm_prove)
+ *      indices_out  (optional) receives the first-round collinearity-check indices; *num_indices in: capacity, out: count.
+ *      Argument and parameter errors return before any kernel is launched. */
+int tvm_fri_prove(tvm_ctx *ctx, uint32_t security_level, uint32_t soundness, uint32_t log2_initial_expansion_factor,
+                  uint32_t log2_high_degree_bound, const uint64_t *codeword, size_t codeword_len, uint64_t *proof_out, size_t *proof_len,
+                  uint32_t *indices_out, size_t *num_indices);
+/* host code, no GPU; TVM_OK = accepted, TVM_ERR_VERIFICATION = rejected (`failure` names the LdtVerificationError variant);
+ * on acceptance the verifier's postscript: first-round indices and the partial first codeword [count][3] (optional outputs).
+ * An initial domain of 2^32 points is TVM_ERR_DOMAIN: the proof stream samples indices below u32::MAX only
+ * (proof_stream.rs:85-89). */
+int tvm_fri_verify(uint32_t security_level, uint32_t soundness, uint32_t log2_initial_expansion_factor, uint32_t log2_high_degree_bound,
+                   const uint64_t *proof, size_t proof_len, uint32_t *indices_out, uint64_t *values_out, size_t *num_indices,
+                   char *failure, size_t failure_capacity);
 /* ---- auxiliary table: MasterMainTable::extend (master_table.rs:1006-1075) = the nine tables' `extend`
  *      (TraceTable::extend, table.rs:29-48; e.g. processor.rs:97-137, hash.rs:304-460, ram.rs:105-255) followed by
  *      DegreeLoweringTable::fill_derived_aux_columns (substitutions.rs:163-205).  SURVEY.md 8(f).1: the stage a host

@@ -420,8 +420,8 @@ int tvm_derive_domains(const tvm_params *p, uint64_t padded_height, tvm_domains 
   if (rc) return rc;
   out->padded_height = d.padded_height; out->num_trace_randomizers = d.num_trace_randomizers;
   out->randomized_trace_len = d.randomized_trace_len; out->trace_len = d.trace_len; out->quotient_len = d.quotient_len;
-  out->ldt_len = d.ldt_len; out->ldt_offset = d.ldt_offset; out->num_collinearity_checks = d.num_collinearity_checks;
-  out->fri_num_rounds = d.fri_num_rounds; out->fri_last_round_max_degree = d.fri_last_round_max_degree;
+  out->ldt_len = d.ldt_len; out->ldt_offset = d.ldt_offset; out->num_collinearity_checks = d.fri.num_collinearity_checks;
+  out->fri_num_rounds = d.fri.num_rounds; out->fri_last_round_max_degree = d.fri.last_round_max_degree;
   out->num_quotient_randomizer_coefficients = d.num_quotient_randomizer_coefficients;
   out->ldt = (uint64_t)d.ldt; out->num_first_round_queries = d.num_first_round_queries;
   out->stir_num_rounds = d.ldt == 2 ? (uint64_t)d.stir.num_rounds : 0;
@@ -680,6 +680,58 @@ int tvm_stir_prove(tvm_ctx *ctx, uint32_t security_level, uint32_t soundness, ui
     deinterleave3_run(c, d_in, d_cw, len, 1);
     ProofStream ps;
     revealed = stir_prove_run(c, mem, ps, d_cw, len, to_mont(7), sd, d_tmp);
+    proof = ps.encode();
+  }
+  const size_t icap = num_indices ? *num_indices : 0;
+  if (num_indices) *num_indices = revealed.size();
+  if (indices_out) {
+    if (icap < revealed.size()) throw ApiError{TVM_ERR_INVALID_ARG, "index buffer too small"};
+    memcpy(indices_out, revealed.data(), revealed.size() * sizeof(uint32_t));
+  }
+  const size_t cap = *proof_len;
+  *proof_len = proof.size();
+  if (!proof_out || cap < proof.size()) throw ApiError{TVM_ERR_INVALID_ARG, "proof buffer too small"};
+  memcpy(proof_out, proof.data(), proof.size() * 8);
+  TVM_API_END
+}
+
+int tvm_fri_derive(uint32_t security_level, uint32_t soundness, uint32_t log2_initial_expansion_factor, uint32_t log2_high_degree_bound,
+                   tvm_fri_info *out) {
+  if (!out || soundness > 1) return TVM_ERR_INVALID_ARG;
+  FriDerived fd{};
+  if (int rc = fri_derive(security_level, soundness == 1, log2_initial_expansion_factor, log2_high_degree_bound, fd)) return rc;
+  out->domain_len = fd.domain_len; out->domain_offset = fd.domain_offset; out->expansion_factor = fd.expansion_factor;
+  out->max_degree = fd.max_degree; out->num_collinearity_checks = fd.num_collinearity_checks; out->num_rounds = fd.num_rounds;
+  out->last_round_max_degree = fd.last_round_max_degree;
+  return TVM_OK;
+}
+
+int tvm_fri_prove(tvm_ctx *ctx, uint32_t security_level, uint32_t soundness, uint32_t log2_initial_expansion_factor,
+                  uint32_t log2_high_degree_bound, const uint64_t *codeword, size_t codeword_len, uint64_t *proof_out, size_t *proof_len,
+                  uint32_t *indices_out, size_t *num_indices) {
+  if (!ctx || !codeword || !proof_len || soundness > 1) return TVM_ERR_INVALID_ARG;
+  TVM_API_BEGIN(ctx)
+  Ctx &c = *c__;
+  FriDerived fd{};
+  const char *why = "";
+  if (int rc = fri_derive(security_level, soundness == 1, log2_initial_expansion_factor, log2_high_degree_bound, fd, &why))
+    throw ApiError{rc, why};
+  if (log2_high_degree_bound + log2_initial_expansion_factor > 26)
+    throw ApiError{TVM_ERR_DOMAIN, "FRI: the device prover supports initial domains of up to 2^26 points"};
+  const size_t len = fd.domain_len;
+  if (codeword_len != len)   // LdtProvingError, fri.rs:323-330
+    throw ApiError{TVM_ERR_INVALID_ARG, "InitialCodewordMismatch { domain_len: " + std::to_string(len) + ", codeword_len: " +
+                                            std::to_string(codeword_len) + " }"};
+  std::vector<u64> proof;
+  std::vector<uint32_t> revealed;
+  {
+    DevMem mem(c);
+    u64 *d_in = mem.words(3 * len), *d_cw = mem.words(3 * len);
+    TVM_CUDA(cudaMemcpyAsync(d_in, codeword, 3 * len * 8, cudaMemcpyDefault, c.stream));
+    to_mont_run(c, d_in, 3 * len);
+    deinterleave3_run(c, d_in, d_cw, len, 1);
+    ProofStream ps;
+    revealed = fri_prove_run(c, mem, ps, d_cw, len, to_mont(fd.domain_offset), fd, d_in /* free again: scratch */);
     proof = ps.encode();
   }
   const size_t icap = num_indices ? *num_indices : 0;

@@ -60,5 +60,9 @@ struct ProofStream;
 // `ps` and returns the revealed first-round indices.
 std::vector<uint32_t> stir_prove_run(Ctx &c, DevMem &mem, ProofStream &ps, const u64 *d_codeword, size_t len, u64 offset_mont,
                                      const StirDerived &sd, u64 *d_tmp /* >= 3*len words */);
+// FRI prover (fri.rs:212-366, 754-772) on a device-resident codeword [3 planes][len] in natural order, Montgomery form, on the
+// domain offset_mont * <g_len>; enqueues into `ps` and returns the first-round collinearity-check indices.
+std::vector<uint32_t> fri_prove_run(Ctx &c, DevMem &mem, ProofStream &ps, const u64 *d_codeword, size_t len, u64 offset_mont,
+                                    const FriDerived &fd, u64 *d_tmp /* >= 3*len words */);
 
 }  // namespace tvm

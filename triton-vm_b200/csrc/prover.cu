@@ -1,7 +1,7 @@
 // Stark::prove on one GPU: orchestration of the device kernels + host Fiat-Shamir transcript.
 //
 // Restates Prover::prove (triton-vm/src/stark.rs:331-719) step by step for the cached-LDE branch
-// with the FRI low-degree test (stark.with_ldt_choice(LdtChoice::Fri); STIR: csrc/stir.cu) and
+// with either low-degree test (FRI: csrc/fri.cu; STIR: csrc/stir.cu) and
 // the parameter derivation of stark.rs:1885-2089, fri.rs:799-924, low_degree_test/mod.rs:250-300.
 // Trace generation stays with the caller (SURVEY.md §8(b)): the main trace and all randomizer
 // coefficients are inputs; the auxiliary trace is requested through a callback once the
@@ -47,7 +47,9 @@ double rs_q_ary_entropy(unsigned log2_exp) {                         // mod.rs:2
 // `conj`: ProximityRegime::Conjectured instead of ::Proven (mod.rs:60-80, 243-287)
 double rs_margin(unsigned log2_exp, bool conj) { return conj ? rs_q_ary_entropy(log2_exp) : std::sqrt(rs_rate(log2_exp)); }
 double rs_slackness(unsigned log2_exp, bool conj) { return rs_margin(log2_exp, conj) / 20.0; }
+}  // namespace
 double rs_proximity_parameter(unsigned log2_exp, bool conj) { return 1.0 - rs_margin(log2_exp, conj) - rs_slackness(log2_exp, conj); }
+namespace {
 double rs_log2_list_size(unsigned log2_exp, bool conj, unsigned log2_poly_degree) {
   const double ls = conj ? std::pow(2.0, (double)log2_poly_degree) / (rs_q_ary_entropy(log2_exp) * rs_slackness(log2_exp, conj))
                          : 1.0 / (2.0 * std::sqrt(rs_rate(log2_exp)) * rs_slackness(log2_exp, conj));
@@ -116,17 +118,14 @@ int stark_derive(const StarkParams &sp, size_t padded_height, StarkDerived &d) {
   const int log2_ph = ilog2(padded_height);
   d = StarkDerived{};
   d.ldt = sp.ldt_choice ? (int)sp.ldt_choice : (log2_ph < (conj ? 17 : 16) ? 1 : 2);      // stark.rs:1942-1951
-  // low_degree_test/mod.rs:243-256 and fri.rs:832-836
-  const double proximity_parameter = rs_proximity_parameter(sp.log2_expansion, conj);
-  const size_t checks = (size_t)std::ceil(-(double)sp.security_level / std::log2(1.0 - proximity_parameter));
   const size_t expansion = (size_t)1 << sp.log2_expansion;
   size_t h = 0, nqr = 0, rtl = 0, ldt_len = 0;
   int hdb = log2_ph;
   for (;;) {                                                             // stark.rs:1972-2060
     hdb++;
-    if (hdb + (int)sp.log2_expansion > 32) return TVM_ERR_LDT_PARAMS;
-    ldt_len = (size_t)1 << (hdb + sp.log2_expansion);
-    size_t first_round = checks;
+    if (int rc = fri_derive(sp.security_level, conj, sp.log2_expansion, (unsigned)hdb, d.fri)) return rc;   // Stark::fri
+    ldt_len = d.fri.domain_len;
+    size_t first_round = d.fri.num_collinearity_checks;
     if (d.ldt == 2) {
       int rc = stir_derive(sp.security_level, STIR_LOG2_FOLDING_FACTOR, sp.log2_expansion, (unsigned)hdb, conj, d.stir);
       if (rc) return rc;
@@ -148,19 +147,13 @@ int stark_derive(const StarkParams &sp, size_t padded_height, StarkDerived &d) {
   upd(AIR_DEGREES_TRAN, AIR_NUM_TRAN, (long long)padded_height - 1);
   upd(AIR_DEGREES_TERM, AIR_NUM_TERM, 1);
   const size_t max_degree = next_pow2((size_t)max_cd) - 1;              // stark.rs:1905-1916
-  const size_t fri_max_degree = ldt_len / expansion - 1;                 // fri.rs:885-887
-  const int max_num_rounds = ilog2(next_pow2(fri_max_degree + 1));
-  const int skip = (checks ? ilog2(checks) : 0) + 1;                     // fri.rs:907-920
   d.padded_height = padded_height;
   d.num_trace_randomizers = h;
   d.randomized_trace_len = rtl;
   d.trace_len = rtl / 2;
   d.quotient_len = next_pow2(max_degree);
   d.ldt_len = ldt_len;
-  d.ldt_offset = 7;                                                      // BFieldElement::generator(), fri.rs:829
-  d.num_collinearity_checks = checks;
-  d.fri_num_rounds = max_num_rounds > skip ? (size_t)(max_num_rounds - skip) : 0;
-  d.fri_last_round_max_degree = fri_max_degree >> d.fri_num_rounds;
+  d.ldt_offset = d.fri.domain_offset;
   d.num_quotient_randomizer_coefficients = nqr;
   return TVM_OK;
 }
@@ -688,82 +681,8 @@ void stark_prove(Ctx &c, const StarkParams &sp, const ClaimView &claim, size_t p
   const size_t max_open = std::max<size_t>(d.num_first_round_queries, 1);
   unsigned *d_idx = (unsigned *)mem.words(max_open * 64 + 64);
   u64 *d_gather = mem.words(max_open * 400 + max_open * 5 * 40 + 64);
-  if (d.ldt == 2) {
-    a_indices = stir_prove_run(c, mem, ps, d_fri, N, off, d.stir, d_tmp);
-  } else {
-  // FRI (fri.rs:212-366, 754-772)
-  struct Round { u64 *cw; size_t len; u64 *nodes; u64 offset; };
-  std::vector<Round> rounds;
-  {
-    u64 *cur = d_fri;
-    size_t len = N;
-    u64 offset = off;
-    for (size_t r = 0; r <= d.fri_num_rounds; r++) {
-      if (r > 0) {
-        xfe chal = ps.sample_scalars(1)[0];
-        u64 *nxt = mem.words(3 * (len / 2));
-        fri_fold_run(c, cur, len, len, offset, chal, nxt, len / 2);
-        cur = nxt; len /= 2; offset = fmul(offset, offset);
-      }
-      u64 *nodes = mem.words(2 * len * 5);
-      TVM_CUDA(cudaMemsetAsync(nodes, 0, 40, c.stream));
-      fri_leaves_run(c, cur, len, len, nodes + 5 * len);
-      merkle_run(c, nodes, len);
-      std::vector<u64> root = d2h(c, nodes + 5, 5);
-      for (auto &v : root) v = from_mont(v);
-      ps.enqueue(ItemKind::MerkleRoot, root);
-      rounds.push_back({cur, len, nodes, offset});
-    }
-  }
-  {
-    const Round &last = rounds.back();
-    std::vector<u64> planes = d2h(c, last.cw, 3 * last.len);
-    std::vector<u64> payload;
-    payload.push_back(last.len);
-    for (size_t i = 0; i < last.len; i++)
-      for (int dd = 0; dd < 3; dd++) payload.push_back(from_mont(planes[dd * last.len + i]));
-    ps.enqueue(ItemKind::FriCodeword, payload);
-    // last polynomial: interpolant over the unit-offset domain of that length (fri.rs:255-268)
-    u64 *d_lp = mem.words(3 * last.len);
-    u64 *d_lp_tmp = mem.words(3 * last.len);
-    NttJob inv{};
-    inv.in = last.cw; inv.in_cstride = last.len; inv.out = d_lp; inv.out_cstride = last.len; inv.tmp = d_lp_tmp;
-    inv.log_n = ilog2(last.len); inv.ncols = 3; inv.inverse = true;
-    ntt_run(c, inv);
-    std::vector<u64> co = d2h(c, d_lp, 3 * last.len);
-    size_t deg_plus_1 = last.len;
-    while (deg_plus_1 > 0 && co[deg_plus_1 - 1] == 0 && co[last.len + deg_plus_1 - 1] == 0 && co[2 * last.len + deg_plus_1 - 1] == 0) deg_plus_1--;
-    // Polynomial { coefficients } encodes like a one-field struct: the coefficient Vec's encoding (count, elements) behind
-    // its own length — pinned by the reference's whole-proof digest (tests/test_golden.py, proof.rs:200-226)
-    payload.clear();
-    payload.push_back(1 + 3 * deg_plus_1);
-    payload.push_back(deg_plus_1);
-    for (size_t i = 0; i < deg_plus_1; i++)
-      for (int dd = 0; dd < 3; dd++) payload.push_back(from_mont(co[dd * last.len + i]));
-    ps.enqueue(ItemKind::Polynomial, payload);
-  }
-  a_indices = ps.sample_indices((uint32_t)N, d.num_collinearity_checks);
-  auto reveal = [&](const Round &rd, const std::vector<uint32_t> &idx) {
-    TVM_CUDA(cudaMemcpyAsync(d_idx, idx.data(), idx.size() * 4, cudaMemcpyHostToDevice, c.stream));
-    gather_rows_run(c, rd.cw, rd.len, 3, d_idx, (unsigned)idx.size(), 0, -1, d_gather);
-    std::vector<u64> leaves = d2h(c, d_gather, idx.size() * 3);
-    std::vector<unsigned> nodes = auth_structure_node_indices(rd.len, idx);
-    std::vector<u64> auth;
-    if (!nodes.empty()) {
-      TVM_CUDA(cudaMemcpyAsync(d_idx, nodes.data(), nodes.size() * 4, cudaMemcpyHostToDevice, c.stream));
-      gather_digests_run(c, rd.nodes, d_idx, (unsigned)nodes.size(), d_gather);
-      auth = d2h(c, d_gather, nodes.size() * 5);
-    }
-    ps.enqueue(ItemKind::FriResponse, encode_fri_response(leaves, auth));
-  };
-  reveal(rounds[0], a_indices);
-  for (size_t r = 0; r + 1 < rounds.size(); r++) {
-    std::vector<uint32_t> b(a_indices.size());
-    for (size_t i = 0; i < b.size(); i++) b[i] = (uint32_t)(((size_t)a_indices[i] + rounds[r].len / 2) % rounds[r].len);
-    reveal(rounds[r], b);
-  }
-  ps.sample_scalars(1);   // fri.rs:764-769
-  }
+  if (d.ldt == 2) a_indices = stir_prove_run(c, mem, ps, d_fri, N, off, d.stir, d_tmp);
+  else a_indices = fri_prove_run(c, mem, ps, d_fri, N, off, d.fri, d_tmp);
   const unsigned nq = (unsigned)a_indices.size();
   mark();  // 11: FRI
 

@@ -23,16 +23,27 @@ struct StirDerived {          // stir.rs:112-147
   size_t in_domain[STIR_MAX_ROUNDS], out_of_domain[STIR_MAX_ROUNDS];
   size_t final_num_in_domain_queries, final_degree;
 };
+struct FriDerived {           // FriParameters::try_into_fri + Fri::{max_degree, num_rounds, last_round_max_degree} (fri.rs:799-924)
+  size_t domain_len;
+  u64 domain_offset;          // canonical: BFieldElement::generator()
+  size_t expansion_factor, max_degree, num_collinearity_checks, num_rounds, last_round_max_degree;
+};
 struct StarkDerived {
   size_t padded_height, num_trace_randomizers, randomized_trace_len, trace_len, quotient_len, ldt_len;
   u64 ldt_offset;  // canonical
-  size_t num_collinearity_checks, fri_num_rounds, fri_last_round_max_degree, num_quotient_randomizer_coefficients;
+  size_t num_quotient_randomizer_coefficients;
   int ldt;                    // 1 = FRI, 2 = STIR
   size_t num_first_round_queries;
+  FriDerived fri;             // derived for the final domain whichever low-degree test runs (tvm_derive_domains reports it)
   StirDerived stir;
 };
+// the Reed-Solomon code's proximity parameter δ of the regime (low_degree_test/mod.rs:243-320)
+double rs_proximity_parameter(unsigned log2_expansion, bool conjectured);
 int stir_derive(unsigned security_level, unsigned log2_folding_factor, unsigned log2_initial_expansion, unsigned log2_high_degree_bound,
                 bool conjectured, StirDerived &out);
+// TVM_OK or TVM_ERR_LDT_PARAMS; `error` (optional) receives the name of the LdtParameterError variant
+int fri_derive(unsigned security_level, bool conjectured, unsigned log2_initial_expansion, unsigned log2_high_degree_bound, FriDerived &out,
+               const char **error = nullptr);
 int stark_derive(const StarkParams &sp, size_t padded_height, StarkDerived &d);
 
 struct ClaimView {            // proof.rs:68-88, canonical words

@@ -315,12 +315,12 @@ struct LdtResult {
   std::vector<xfe> values;
 };
 
-LdtResult fri_verify(Transcript &ps, const StarkDerived &d) {
-  const size_t checks = d.num_collinearity_checks, num_rounds = d.fri_num_rounds;
+LdtResult fri_verify(Transcript &ps, const FriDerived &d) {
+  const size_t checks = d.num_collinearity_checks, num_rounds = d.num_rounds;
   struct Round { u64 offset; size_t len; std::vector<u64> root; xfe chal; std::vector<xfe> a, b; };
   std::vector<Round> rounds;
-  u64 offset = to_mont(d.ldt_offset);
-  size_t length = d.ldt_len;
+  u64 offset = to_mont(d.domain_offset);
+  size_t length = d.domain_len;
   for (size_t j = 0; j <= num_rounds; j++) {
     Round r;
     r.offset = offset; r.len = length;
@@ -334,19 +334,22 @@ LdtResult fri_verify(Transcript &ps, const StarkDerived &d) {
   std::vector<xfe> last_codeword = ps.xfe_vector(ItemKind::FriCodeword, "UnexpectedItem: FriCodeword");
   std::vector<xfe> last_poly = ps.polynomial();
   if (last_codeword.size() != rounds.back().len) fail("LdtVerificationError: LastCodewordMismatch");
-  std::vector<uint32_t> a_indices = ps.sponge.sample_indices((uint32_t)d.ldt_len, checks);
 
   auto check = [&](size_t rnd, const std::vector<uint32_t> &idx, const std::vector<xfe> &leaves,
                    const std::vector<std::vector<u64>> &auth) {
-    if (leaves.size() != checks) fail("LdtVerificationError: IncorrectNumberOfRevealedLeaves");
     std::vector<std::vector<u64>> lf;
     for (xfe v : leaves) lf.push_back(xfe_leaf(v));
     if (!verify_inclusion(rounds[rnd].root, ilog2z(rounds[rnd].len), idx, lf, auth)) fail("LdtVerificationError: BadMerkleAuthenticationPath");
   };
+  std::vector<uint32_t> a_indices;
   {
+    // The first response is read, and its size checked, before the indices are sampled: responses are outside Fiat-Shamir
+    // (proof_item.rs:140-145), so the order changes no outcome, and the number of indices drawn stays bounded by the proof.
     std::vector<xfe> leaves;
     std::vector<std::vector<u64>> auth;
     ps.fri_response(leaves, auth);
+    if (leaves.size() != checks) fail("LdtVerificationError: IncorrectNumberOfRevealedLeaves");
+    a_indices = ps.sponge.sample_indices((uint32_t)d.domain_len, checks);
     std::vector<uint32_t> idx;
     for (uint32_t a : a_indices) idx.push_back(a % (uint32_t)rounds[0].len);
     check(0, idx, leaves, auth);
@@ -357,6 +360,7 @@ LdtResult fri_verify(Transcript &ps, const StarkDerived &d) {
     std::vector<xfe> leaves;
     std::vector<std::vector<u64>> auth;
     ps.fri_response(leaves, auth);
+    if (leaves.size() != checks) fail("LdtVerificationError: IncorrectNumberOfRevealedLeaves");
     std::vector<uint32_t> idx;
     for (uint32_t a : a_indices) idx.push_back((uint32_t)((a + n / 2) % n));
     check(rnd, idx, leaves, auth);
@@ -389,7 +393,7 @@ LdtResult fri_verify(Transcript &ps, const StarkDerived &d) {
     for (size_t i = 0; i < a_indices.size(); i++)
       if (!xeq(last_codeword[a_indices[i] % nl], rounds.back().a[i])) fail("LdtVerificationError: LastCodewordMismatch");
   }
-  if (!last_poly.empty() && last_poly.size() - 1 > d.fri_last_round_max_degree) fail("LdtVerificationError: LastRoundPolynomialHasTooHighDegree");
+  if (!last_poly.empty() && last_poly.size() - 1 > d.last_round_max_degree) fail("LdtVerificationError: LastRoundPolynomialHasTooHighDegree");
   const xfe x = ps.sponge.sample_scalars(1)[0];
   if (!xeq(xpoly_eval(last_poly, x), barycentric_evaluate(last_codeword, x))) fail("LdtVerificationError: LastRoundPolynomialEvaluationMismatch");
   return {a_indices, rounds[0].a};
@@ -481,7 +485,7 @@ void stark_verify(const StarkParams &sp, const ClaimView &claim, const u64 *proo
     ood_r_value = xadd(ood_r_value, xmul(ood_r[i], w_quot[i + 1]));
   }
 
-  LdtResult ldt = d.ldt == 2 ? stir_verify(ps, d) : fri_verify(ps, d);
+  LdtResult ldt = d.ldt == 2 ? stir_verify(ps, d) : fri_verify(ps, d.fri);
   const size_t q = d.num_first_round_queries;
   if (ldt.indices.size() != q || ldt.values.size() != q) fail("VerificationError: IncorrectNumberOfRowIndices");
 
@@ -735,6 +739,55 @@ extern "C" int tvm_stir_verify(uint32_t security_level, uint32_t soundness, uint
   try {
     Transcript ps(proof, proof_len);
     LdtResult r = stir_verify(ps, d);
+    if (ps.index != ps.items.size()) fail("VerificationError: SuperfluousProofItems");
+    const size_t cap = num_indices ? *num_indices : 0;
+    if (num_indices) *num_indices = r.indices.size();
+    if (indices_out || values_out) {
+      if (cap < r.indices.size()) return TVM_ERR_INVALID_ARG;
+      for (size_t i = 0; i < r.indices.size(); i++) {
+        if (indices_out) indices_out[i] = r.indices[i];
+        if (values_out) { values_out[3 * i] = from_mont(r.values[i].c0); values_out[3 * i + 1] = from_mont(r.values[i].c1); values_out[3 * i + 2] = from_mont(r.values[i].c2); }
+      }
+    }
+    return TVM_OK;
+  } catch (const VerifyFailure &f) {
+    report(f.what);
+    return TVM_ERR_VERIFICATION;
+  } catch (const std::exception &e) {
+    report(e.what());
+    return TVM_ERR_VERIFICATION;
+  } catch (...) {
+    report("internal error");
+    return TVM_ERR_VERIFICATION;
+  }
+}
+
+// Fri::verify as a stand-alone low-degree test (fri.rs:774-789) for arbitrary FriParameters: the fri_verify of tvm_verify
+extern "C" int tvm_fri_verify(uint32_t security_level, uint32_t soundness, uint32_t log2_initial_expansion_factor,
+                              uint32_t log2_high_degree_bound, const uint64_t *proof, size_t proof_len, uint32_t *indices_out,
+                              uint64_t *values_out, size_t *num_indices, char *failure, size_t failure_capacity) {
+  using namespace tvm;
+  if (failure && failure_capacity) failure[0] = 0;
+  if (!proof || !proof_len || soundness > 1) return TVM_ERR_INVALID_ARG;
+  auto report = [&](const char *what) {
+    if (failure && failure_capacity) {
+      std::strncpy(failure, what, failure_capacity - 1);
+      failure[failure_capacity - 1] = 0;
+    }
+  };
+  FriDerived d{};
+  const char *why = "";
+  if (int rc = fri_derive(security_level, soundness == 1, log2_initial_expansion_factor, log2_high_degree_bound, d, &why)) {
+    report(why);
+    return rc;
+  }
+  if (d.domain_len > ((size_t)1 << 31)) {   // ProofStream::sample_indices takes upper bounds up to u32::MAX (proof_stream.rs:85-89)
+    report("ProofStream::sample_indices: upper bound exceeds u32::MAX");
+    return TVM_ERR_DOMAIN;
+  }
+  try {
+    Transcript ps(proof, proof_len);
+    LdtResult r = fri_verify(ps, d);
     if (ps.index != ps.items.size()) fail("VerificationError: SuperfluousProofItems");
     const size_t cap = num_indices ? *num_indices : 0;
     if (num_indices) *num_indices = r.indices.size();

@@ -60,6 +60,11 @@ class Domains(ctypes.Structure):
         return d
 
 
+class FriInfo(ctypes.Structure):   # tvm_fri_info
+    _fields_ = [(n, ctypes.c_uint64) for n in (
+        "domain_len", "domain_offset", "expansion_factor", "max_degree", "num_collinearity_checks", "num_rounds", "last_round_max_degree")]
+
+
 class ClaimStruct(ctypes.Structure):
     _fields_ = [("program_digest", ctypes.c_uint64 * 5), ("version", ctypes.c_uint32), ("input", _u64p),
                 ("num_input", ctypes.c_size_t), ("output", _u64p), ("num_output", ctypes.c_size_t)]
@@ -176,6 +181,11 @@ _SIGNATURES = {
                                       ctypes.POINTER(ctypes.c_size_t), ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_size_t)]),
     "tvm_stir_verify": (ctypes.c_int, [ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, _u64p, ctypes.c_size_t,
                                        ctypes.POINTER(ctypes.c_uint32), _u64p, ctypes.POINTER(ctypes.c_size_t), ctypes.c_char_p, ctypes.c_size_t]),
+    "tvm_fri_derive": (ctypes.c_int, [ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, ctypes.POINTER(FriInfo)]),
+    "tvm_fri_prove": (ctypes.c_int, [_vp, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, _u64p, ctypes.c_size_t, _u64p,
+                                     ctypes.POINTER(ctypes.c_size_t), ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_size_t)]),
+    "tvm_fri_verify": (ctypes.c_int, [ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, _u64p, ctypes.c_size_t,
+                                      ctypes.POINTER(ctypes.c_uint32), _u64p, ctypes.POINTER(ctypes.c_size_t), ctypes.c_char_p, ctypes.c_size_t]),
     "tvm_fill_derived_main_columns": (ctypes.c_int, [_vp, _u64p, ctypes.c_uint]),
     "tvm_aux_extend": (ctypes.c_int, [_vp, _u64p, ctypes.c_uint, _u64p, _u64p, _u64p]),
     "tvm_verify": (ctypes.c_int, [ctypes.POINTER(Params), ctypes.POINTER(ClaimStruct), _u64p, ctypes.c_size_t, ctypes.c_int,
@@ -219,6 +229,35 @@ def stir_verify(security_level, log2_expansion, log2_high_degree_bound, proof, c
     if rc == -9:
         return False, msg.value.decode(), [], vals[:0]
     raise TvmError(rc, lib().tvm_strerror(rc).decode())
+
+
+def fri_derive(security_level, log2_expansion, log2_high_degree_bound, conjectured=False):
+    """FriParameters::try_into_fri + Fri::{max_degree, num_rounds, last_round_max_degree} (host code, no GPU) -> dict of
+    tvm_fri_info's fields; raises TvmError (TVM_ERR_LDT_PARAMS = -6) for parameters the reference rejects"""
+    out = FriInfo()
+    rc = lib().tvm_fri_derive(security_level, int(conjectured), log2_expansion, log2_high_degree_bound, ctypes.byref(out))
+    if rc:
+        raise TvmError(rc, lib().tvm_strerror(rc).decode())
+    return {n: int(getattr(out, n)) for n, _ in FriInfo._fields_}
+
+
+def fri_verify(security_level, log2_expansion, log2_high_degree_bound, proof, conjectured=False):
+    """Fri::verify for arbitrary FriParameters (host code, no GPU) -> (accepted, failure, first-round indices, partial first
+    codeword [k,3]).  Parameter errors raise TvmError."""
+    pr, prp = _np_u64(proof)
+    cap = 1 << 16
+    icap = ctypes.c_size_t(cap)
+    idx = (ctypes.c_uint32 * cap)()
+    vals = np.zeros((cap, 3), dtype=np.uint64)
+    msg = ctypes.create_string_buffer(256)
+    rc = lib().tvm_fri_verify(security_level, int(conjectured), log2_expansion, log2_high_degree_bound, prp, pr.size, idx,
+                              vals.ctypes.data_as(_u64p), ctypes.byref(icap), msg, 256)
+    if rc == 0:
+        k = icap.value
+        return True, "", [int(idx[i]) for i in range(k)], vals[:k].copy()
+    if rc == -9:
+        return False, msg.value.decode(), [], vals[:0]
+    raise TvmError(rc, lib().tvm_strerror(rc).decode() + " | " + msg.value.decode())
 
 
 def _proof_capacity(dom):
@@ -719,6 +758,26 @@ class Backend:
         cap.value = est
         self._chk(self._l.tvm_stir_prove(self._h, security_level, int(conjectured), log2_expansion, log2_high_degree_bound, cwp,
                                          buf.ctypes.data_as(_u64p), ctypes.byref(cap), idx, ctypes.byref(icap)))
+        return buf[:cap.value].copy(), [int(idx[i]) for i in range(icap.value)]
+
+    def fri_prove(self, security_level, log2_expansion, log2_high_degree_bound, codeword, conjectured=False):
+        """Fri::prove on the device for arbitrary FriParameters: codeword [2^(hdb+exp), 3] canonical (numpy, or a contiguous torch
+        tensor on the host or the device) -> (proof words, first-round indices)"""
+        cw, cwp, shape = _u64_arg(codeword)
+        n = int(np.prod(shape)) // 3
+        try:
+            fd = fri_derive(security_level, log2_expansion, log2_high_degree_bound, conjectured)
+        except TvmError:
+            fd = dict(num_collinearity_checks=0, num_rounds=0, domain_len=0)   # tvm_fri_prove names the parameter error
+        checks, rounds = fd["num_collinearity_checks"], fd["num_rounds"]
+        # roots, last codeword and polynomial, one response per round: leaves plus at most checks * height digests
+        est = 64 + 8 * (rounds + 1) + 6 * (fd["domain_len"] >> rounds) + (rounds + 1) * (8 + checks * (3 + 5 * fd["domain_len"].bit_length()))
+        buf = np.empty(est, dtype=np.uint64)
+        cap = ctypes.c_size_t(est)
+        icap = ctypes.c_size_t(max(1, checks))
+        idx = (ctypes.c_uint32 * max(1, checks))()
+        self._chk(self._l.tvm_fri_prove(self._h, security_level, int(conjectured), log2_expansion, log2_high_degree_bound, cwp, n,
+                                        buf.ctypes.data_as(_u64p), ctypes.byref(cap), idx, ctypes.byref(icap)))
         return buf[:cap.value].copy(), [int(idx[i]) for i in range(icap.value)]
 
     def set_low_memory(self, mode):
