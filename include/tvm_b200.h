@@ -285,6 +285,49 @@ int tvm_prove_aet_seeded(tvm_ctx *ctx, const tvm_params *params, const tvm_claim
 int tvm_prove_tables_seeded(tvm_ctx *ctx, const tvm_params *params, const tvm_claim *claim, uint64_t padded_height,
                             const uint64_t *main_table, int fill_derived_main_columns, const uint8_t seed[32], uint64_t *proof_out,
                             size_t *proof_len);
+/* ---- Proving a program from its inputs: VM::trace_execution (vm.rs:159-196) and triton_vm::prove_program (lib.rs:228-267).
+ *      tvm_trace_execution runs the program on the host and keeps what AlgebraicExecutionTrace (aet.rs:41-91) records, except
+ *      the three Hash-table traces: of those only the 16-word input state of every Tip5 permutation is kept, and the traces
+ *      (67 columns, 6 rows per permutation) are expanded on the device when they are needed.
+ *        program      Program::to_bwords() (no length prefix), decoded as Program::decode (program.rs:65-108) decodes it
+ *        public_input PublicInput; nd: NonDeterminism (vm.rs:1467-1471), NULL = empty
+ *      Words >= p in the program, inputs, digests or RAM, and a RAM address given twice, are TVM_ERR_INVALID_ARG.  A program
+ *      the VM rejects is TVM_ERR_VM; `failure` (optional) then names the reference's variant and, for a VMError, the clock
+ *      cycle and instruction pointer: "VMError: AssertionFailed (clk 17, ip 9)", "ProgramDecodingError: MissingArgument(6, push)".
+ *      DIVERGENCE: the reference runs a program that never halts until memory is exhausted.  Here execution stops with
+ *      TVM_ERR_DOMAIN as soon as any table would grow beyond 2^26 rows, the largest height tvm_main_table_from_aet takes: nothing
+ *      taller can be proved by this library.
+ *      The execution is host memory only; any number of contexts may use it concurrently. --- */
+#define TVM_ERR_VM (-10)          /* VMError / ProgramDecodingError: the program cannot be executed */
+#define TVM_CURRENT_VERSION 6     /* proof.rs:33; the version tvm_prove_execution puts into the claim (Claim::new) */
+typedef struct tvm_nondeterminism {                                     /* NonDeterminism (vm.rs:1467-1471) */
+  const uint64_t *individual_tokens; size_t num_individual_tokens;     /* secret input, consumed by `divine` */
+  const uint64_t *digests; size_t num_digests;                         /* [num_digests][5], consumed by `merkle_step` */
+  const uint64_t *ram_addresses, *ram_values; size_t num_ram;          /* initial RAM */
+} tvm_nondeterminism;
+typedef struct tvm_execution tvm_execution;
+typedef struct tvm_execution_summary {
+  uint64_t program_digest[5];   /* Program::hash */
+  uint64_t padded_height;       /* AlgebraicExecutionTrace::padded_height (aet.rs:133-146) */
+  uint64_t table_heights[9];    /* height_of_table, in the order of tvm_main_table_from_aet's table_lengths_out */
+  uint64_t num_output;
+} tvm_execution_summary;
+/* host code, no GPU */
+int tvm_trace_execution(const uint64_t *program, size_t program_len, const uint64_t *public_input, size_t num_input,
+                        const tvm_nondeterminism *nd, tvm_execution **out, char *failure, size_t failure_capacity);
+/* output: [num_output] public output, or NULL */
+int tvm_execution_info(const tvm_execution *ex, tvm_execution_summary *out, uint64_t *output);
+/* the reference's AET as tvm_aet: pointers into storage owned by `ex`, valid until tvm_execution_destroy.  The three hash traces
+ * are expanded on the device of `ctx` (and kept with `ex`); with ctx == NULL they are NULL, their row counts are still set. */
+int tvm_execution_aet(tvm_ctx *ctx, const tvm_execution *ex, tvm_aet *out);
+/* Stark::prove(Claim::new(digest).with_input(input).with_output(output), aet) with Prover::prove's randomness drawn from `seed`:
+ * the proof words tvm_prove_aet_seeded gives for that claim (version TVM_CURRENT_VERSION), tvm_execution_aet's AET and the
+ * execution's padded height.  The hash traces are expanded into device memory and never cross PCIe.  The proof-capacity
+ * protocol is tvm_prove's; a retry proves again but does not execute again.  With tvm_ctx_set_comm every rank traces the same
+ * inputs itself and calls this with the same seed.  The seed WARNING of the seeded entry points applies. */
+int tvm_prove_execution(tvm_ctx *ctx, const tvm_params *params, const tvm_execution *ex, const uint8_t seed[32],
+                        uint64_t *proof_out, size_t *proof_len);
+void tvm_execution_destroy(tvm_execution *ex);
 /* Bezout coefficient polynomials of rp = prod (x - roots[i]) and its formal derivative (ram.rs:162-214), kernel-level entry
  * point: `roots` m distinct canonical elements; a_out, b_out [m] canonical coefficients, lowest first. */
 int tvm_bezout_coefficients(tvm_ctx *ctx, const uint64_t *roots, uint64_t m, uint64_t *a_out, uint64_t *b_out);

@@ -5,7 +5,10 @@
 #include "transcript.h"
 #include "prove_common.h"
 #include "stark.h"
+#include "vm.h"
+#include <algorithm>
 #include <cstring>
+#include <memory>
 #include <new>
 #include <stdexcept>
 
@@ -236,6 +239,7 @@ const char *tvm_strerror(int code) {
     case TVM_ERR_STATE: return "entry point called out of order";
     case TVM_ERR_UNSUPPORTED: return "unsupported configuration";
     case TVM_ERR_VERIFICATION: return "proof rejected (VerificationError)";
+    case TVM_ERR_VM: return "the program cannot be executed (VMError / ProgramDecodingError)";
     default: return "unknown error";
   }
 }
@@ -635,6 +639,133 @@ int tvm_prove_tables_seeded(tvm_ctx *ctx, const tvm_params *params, const tvm_cl
   memcpy(proof_out, proof.data(), proof.size() * 8);
   TVM_API_END
 }
+
+static void set_failure(char *failure, size_t capacity, const std::string &text) {
+  if (!failure || !capacity) return;
+  const size_t n = std::min(capacity - 1, text.size());
+  memcpy(failure, text.data(), n);
+  failure[n] = 0;
+}
+
+int tvm_trace_execution(const uint64_t *program, size_t program_len, const uint64_t *public_input, size_t num_input,
+                        const tvm_nondeterminism *nd, tvm_execution **out, char *failure, size_t failure_capacity) {
+  set_failure(failure, failure_capacity, "");
+  if (!out) return TVM_ERR_INVALID_ARG;
+  *out = nullptr;
+  static const tvm_nondeterminism empty{};
+  if (!nd) nd = &empty;
+  if ((program_len && !program) || (num_input && !public_input) || (nd->num_individual_tokens && !nd->individual_tokens) ||
+      (nd->num_digests && !nd->digests) || (nd->num_ram && (!nd->ram_addresses || !nd->ram_values)))
+    return TVM_ERR_INVALID_ARG;
+  auto canonical = [](const uint64_t *w, size_t n) {
+    for (size_t i = 0; i < n; i++) if (w[i] >= P) return false;
+    return true;
+  };
+  if (!canonical(program, program_len) || !canonical(public_input, num_input) ||
+      !canonical(nd->individual_tokens, nd->num_individual_tokens) || !canonical(nd->digests, 5 * nd->num_digests) ||
+      !canonical(nd->ram_addresses, nd->num_ram) || !canonical(nd->ram_values, nd->num_ram)) {
+    set_failure(failure, failure_capacity, "a word is not a canonical field element (>= p)");
+    return TVM_ERR_INVALID_ARG;
+  }
+  try {
+    std::vector<uint64_t> addresses(nd->ram_addresses, nd->ram_addresses + nd->num_ram);
+    std::sort(addresses.begin(), addresses.end());
+    if (std::adjacent_find(addresses.begin(), addresses.end()) != addresses.end()) {
+      set_failure(failure, failure_capacity, "a RAM address is given twice");
+      return TVM_ERR_INVALID_ARG;
+    }
+    std::unique_ptr<tvm_execution> ex(new tvm_execution());
+    std::string why;
+    const VmInputs in{program, program_len, public_input, num_input, nd->individual_tokens, nd->num_individual_tokens,
+                      nd->digests, nd->num_digests, nd->ram_addresses, nd->ram_values, nd->num_ram};
+    if (int rc = trace_execution(in, *ex, why)) {
+      set_failure(failure, failure_capacity, why);
+      return rc;
+    }
+    *out = ex.release();
+    return TVM_OK;
+  } catch (const std::bad_alloc &) {
+    set_failure(failure, failure_capacity, "host allocation failed");
+    return TVM_ERR_OOM;
+  }
+}
+
+int tvm_execution_info(const tvm_execution *ex, tvm_execution_summary *out, uint64_t *output) {
+  if (!ex || !out) return TVM_ERR_INVALID_ARG;
+  memcpy(out->program_digest, ex->digest, sizeof ex->digest);
+  out->padded_height = ex->padded_height;
+  memcpy(out->table_heights, ex->table_heights, sizeof ex->table_heights);
+  out->num_output = ex->output.size();
+  if (output && !ex->output.empty()) memcpy(output, ex->output.data(), ex->output.size() * 8);
+  return TVM_OK;
+}
+
+// the execution's AET with host arrays; the three hash traces NULL
+static tvm_aet execution_aet_host(const tvm_execution &ex) {
+  tvm_aet a{};
+  a.program = ex.program.data(); a.program_len = ex.program.size();
+  a.instruction_multiplicities = ex.instruction_multiplicities.data();
+  a.processor_trace = ex.processor_trace.data(); a.processor_rows = ex.processor_trace.size() / 39;
+  a.op_stack_underflow_trace = ex.op_stack_trace.data(); a.op_stack_rows = ex.op_stack_trace.size() / 4;
+  a.ram_trace = ex.ram_trace.data(); a.ram_rows = ex.ram_trace.size() / 7;
+  a.program_hash_rows = ex.hash_rows[0]; a.sponge_rows = ex.hash_rows[1]; a.hash_rows = ex.hash_rows[2];
+  a.u32_entries = ex.u32_entries.data(); a.u32_count = ex.u32_entries.size() / 4;
+  a.cascade_table_lookup_multiplicities = ex.cascade_multiplicities.data(); a.cascade_count = ex.cascade_multiplicities.size() / 2;
+  a.lookup_table_lookup_multiplicities = ex.lookup_multiplicities;
+  return a;
+}
+
+int tvm_execution_aet(tvm_ctx *ctx, const tvm_execution *ex, tvm_aet *out) {
+  if (!ex || !out) return TVM_ERR_INVALID_ARG;
+  *out = execution_aet_host(*ex);
+  if (!ctx) return TVM_OK;
+  TVM_API_BEGIN(ctx)
+  Ctx &c = *c__;
+  if (!ex->expanded) {
+    DevMem mem(c);
+    u64 *d[3];
+    hash_trace_run(c, mem, *ex, d);
+    for (int s = 0; s < 3; s++) {
+      ex->hash_cache[s].resize(ex->hash_rows[s] * 67);
+      if (ex->hash_rows[s])
+        TVM_CUDA(cudaMemcpyAsync(ex->hash_cache[s].data(), d[s], ex->hash_cache[s].size() * 8, cudaMemcpyDeviceToHost, c.stream));
+    }
+    TVM_CUDA(cudaStreamSynchronize(c.stream));
+    ex->expanded = true;
+  }
+  out->program_hash_trace = ex->hash_cache[0].data();
+  out->sponge_trace = ex->hash_cache[1].data();
+  out->hash_trace = ex->hash_cache[2].data();
+  TVM_API_END
+}
+
+int tvm_prove_execution(tvm_ctx *ctx, const tvm_params *params, const tvm_execution *ex, const uint8_t seed[32], uint64_t *proof_out,
+                        size_t *proof_len) {
+  if (!ctx || !params || !ex || !seed || !proof_len || params->ldt_choice > 2) return TVM_ERR_INVALID_ARG;
+  TVM_API_BEGIN(ctx)
+  const StarkParams sp{params->security_level, params->log2_ldt_expansion_factor, params->ldt_choice, params->soundness};
+  StarkDerived derived{};
+  if (int rc = stark_derive(sp, ex->padded_height, derived)) throw ApiError{rc, "parameter derivation failed"};
+  const ClaimView cv{ex->digest, TVM_CURRENT_VERSION, ex->input.data(), ex->input.size(), ex->output.data(), ex->output.size()};
+  std::vector<u64> proof;
+  {
+    DevMem mem(*c__);
+    tvm_aet a = execution_aet_host(*ex);
+    u64 *d[3];
+    hash_trace_run(*c__, mem, *ex, d);
+    a.program_hash_trace = d[0]; a.sponge_trace = d[1]; a.hash_trace = d[2];
+    const SeededRandomness r = seeded_randomness(*c__, mem, sp, ex->padded_height, seed);
+    DeviceTables dt{r.aux_rand, r.randomizer_column, true, &a};
+    stark_prove(*c__, sp, cv, ex->padded_height, nullptr, r.main_rand, nullptr, nullptr, r.quot_rand, proof, &ctx->timings, &dt);
+  }
+  size_t cap = *proof_len;
+  *proof_len = proof.size();
+  if (!proof_out || cap < proof.size()) throw ApiError{TVM_ERR_INVALID_ARG, "proof buffer too small"};
+  memcpy(proof_out, proof.data(), proof.size() * 8);
+  TVM_API_END
+}
+
+void tvm_execution_destroy(tvm_execution *ex) { delete ex; }
 
 int tvm_bezout_coefficients(tvm_ctx *ctx, const uint64_t *roots, uint64_t m, uint64_t *a_out, uint64_t *b_out) {
   if (!ctx || (m && (!roots || !a_out || !b_out))) return TVM_ERR_INVALID_ARG;

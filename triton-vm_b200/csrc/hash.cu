@@ -959,6 +959,10 @@ void tip5_permutation_host(u64 s[16]) {
   u64(&st)[16] = *reinterpret_cast<u64(*)[16]>(s);
   tip5_permutation_generic(st, HostLutF{}, HostRcF{});
 }
+void tip5_round_host(u64 s[16], int rnd) {
+  u64(&st)[16] = *reinterpret_cast<u64(*)[16]>(s);
+  tip5_round_generic(st, rnd, HostLutF{}, HostRcF{});
+}
 void tip5_hash_varlen_host(const u64 *w, size_t n, u64 digest[5]) {
   u64 s[16] = {0};
   size_t full = n / 10;

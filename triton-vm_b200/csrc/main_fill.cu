@@ -10,6 +10,8 @@
 #include "stark.h"
 #include "tip5.cuh"
 #include "fill/main_fill.cuh"
+#include "fill/hash_trace.cuh"
+#include "vm.h"
 
 namespace tvm {
 
@@ -123,6 +125,17 @@ void main_fill_run(Ctx &c, DevMem &mem, const tvm_aet &a, size_t n, u64 *d_table
 void bezout_run(Ctx &c, DevMem &mem, const u64 *d_roots_mont, size_t m, u64 *d_a, u64 *d_b) {
   CudaExec ex{c, mem};
   fill::bezout_coefficients(ex, d_roots_mont, m, d_a, d_b);
+}
+
+void hash_trace_run(Ctx &c, DevMem &mem, const tvm_execution &e, u64 *d_out[3]) {
+  const size_t count = e.perm_meta.size();
+  const std::vector<u64> k = hash_trace::constants(TIP5_ROUND_CONSTANTS_HOST, TIP5_LOOKUP_HOST);
+  const u64 *d_states = upload(c, mem, e.perm_states.data(), 16 * count), *d_meta = upload(c, mem, e.perm_meta.data(), count);
+  const u64 *d_k = upload(c, mem, k.data(), k.size());
+  for (int s = 0; s < 3; s++) d_out[s] = mem.words(e.hash_rows[s] * hash_trace::H_WIDTH);
+  CudaExec ex{c, mem};
+  hash_trace::expand(ex, d_states, d_meta, count, d_k, d_out[0], d_out[1], d_out[2]);
+  TVM_CUDA(cudaStreamSynchronize(c.stream));   // `k` is a pageable host vector of this frame
 }
 
 }  // namespace tvm

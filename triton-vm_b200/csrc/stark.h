@@ -79,6 +79,8 @@ void stark_prove(Ctx &c, const StarkParams &sp, const ClaimView &claim, size_t p
 // ---- main_fill.cu: MasterMainTable::new + pad from the AET; d_table [>= 149][n] receives CANONICAL columns ----
 void main_fill_run(Ctx &c, struct DevMem &mem, const tvm_aet &aet, size_t n, u64 *d_table, uint64_t *lengths9);
 void bezout_run(Ctx &c, struct DevMem &mem, const u64 *d_roots_mont, size_t m, u64 *d_a, u64 *d_b);
+// the three hash traces of an execution (fill/hash_trace.cuh) into device memory of `mem`: d_out[section] [rows][67] canonical
+void hash_trace_run(Ctx &c, struct DevMem &mem, const tvm_execution &ex, u64 *d_out[3]);
 
 // ---- prover_randomness.cu: the prover's four randomness arrays from its 32-byte seed, CANONICAL, concatenated ----
 struct ProverRandomnessLayout {   // word offsets into the concatenation, and its length

@@ -120,6 +120,21 @@ def aet_struct(arrays):
     return s, keep
 
 
+class NondeterminismStruct(ctypes.Structure):   # tvm_nondeterminism (vm.rs:1467-1471)
+    _fields_ = [("individual_tokens", _u64p), ("num_individual_tokens", ctypes.c_size_t), ("digests", _u64p),
+                ("num_digests", ctypes.c_size_t), ("ram_addresses", _u64p), ("ram_values", _u64p), ("num_ram", ctypes.c_size_t)]
+
+
+class ExecutionSummary(ctypes.Structure):   # tvm_execution_summary
+    _fields_ = [("program_digest", ctypes.c_uint64 * 5), ("padded_height", ctypes.c_uint64), ("table_heights", ctypes.c_uint64 * 9),
+                ("num_output", ctypes.c_uint64)]
+
+
+TABLES = ("program", "processor", "op_stack", "ram", "jump_stack", "hash", "cascade", "lookup", "u32")   # table_heights order
+TVM_ERR_VM = -10
+CURRENT_VERSION = 6
+
+
 AUX_CALLBACK = ctypes.CFUNCTYPE(ctypes.c_int, _vp, _u64p, ctypes.POINTER(_u64p), ctypes.POINTER(_u64p))
 ALL_GATHER_CB = ctypes.CFUNCTYPE(ctypes.c_int, _vp, _vp, ctypes.c_size_t, _vp)
 ALL_REDUCE_CB = ctypes.CFUNCTYPE(ctypes.c_int, _vp, _u64p, ctypes.c_size_t, _vp)
@@ -195,6 +210,12 @@ _SIGNATURES = {
                                         ctypes.POINTER(ctypes.c_int)]),
     "tvm_proof_padded_height": (ctypes.c_int, [_u64p, ctypes.c_size_t, ctypes.POINTER(ctypes.c_uint64)]),
     "tvm_last_prove_timings": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_float)]),
+    "tvm_trace_execution": (ctypes.c_int, [_u64p, ctypes.c_size_t, _u64p, ctypes.c_size_t, ctypes.POINTER(NondeterminismStruct),
+                                           ctypes.POINTER(_vp), ctypes.c_char_p, ctypes.c_size_t]),
+    "tvm_execution_info": (ctypes.c_int, [_vp, ctypes.POINTER(ExecutionSummary), _u64p]),
+    "tvm_execution_aet": (ctypes.c_int, [_vp, _vp, ctypes.POINTER(AetStruct)]),
+    "tvm_prove_execution": (ctypes.c_int, [_vp, ctypes.POINTER(Params), _vp, ctypes.c_char_p, _u64p, ctypes.POINTER(ctypes.c_size_t)]),
+    "tvm_execution_destroy": (None, [_vp]),
     "tvm_air_quotient_dev": (ctypes.c_int, [_vp, _vp, ctypes.c_size_t, _vp, ctypes.c_size_t, _u64p, _u64p, ctypes.c_uint,
                                             ctypes.c_uint, ctypes.c_uint64, _vp, ctypes.c_size_t]),
 }
@@ -294,6 +315,89 @@ def hash_varlen(words):
     if rc:
         raise TvmError(rc, lib().tvm_strerror(rc).decode())
     return [int(v) for v in d]
+
+
+def _rows(ptr, count, width, dtype=np.uint64):
+    """copy of `count` rows of `width` words at a ctypes pointer (NULL allowed when count == 0)"""
+    if not count:
+        return np.zeros((0, width) if width else 0, dtype=dtype)
+    n = count * (width or 1)
+    a = np.ctypeslib.as_array(ctypes.cast(ptr, ctypes.POINTER(ctypes.c_uint32 if dtype == np.uint32 else ctypes.c_uint64)), shape=(n,))
+    return a.copy().reshape((count, width) if width else (count,))
+
+
+class Execution:
+    """VM::trace_execution's result (tvm_trace_execution): program digest, padded height, table heights, public output, and the
+    AlgebraicExecutionTrace on demand.  Host memory; `close()` frees it (also on garbage collection)."""
+
+    def __init__(self, handle, public_input):
+        self._l, self._h = lib(), handle
+        s = ExecutionSummary()
+        _check_plain(self._l.tvm_execution_info(self._h, ctypes.byref(s), None))
+        out = np.zeros(max(1, int(s.num_output)), dtype=np.uint64)
+        _check_plain(self._l.tvm_execution_info(self._h, ctypes.byref(s), out.ctypes.data_as(_u64p)))
+        self.program_digest = [int(v) for v in s.program_digest]
+        self.padded_height = int(s.padded_height)
+        self.table_heights = dict(zip(TABLES, (int(v) for v in s.table_heights)))
+        self.input = [int(v) for v in public_input]
+        self.output = [int(v) for v in out[:int(s.num_output)]]
+
+    @property
+    def claim(self):
+        """(program digest, input, output): the claim the other bindings take (Claim::new(digest).with_input().with_output())"""
+        return (self.program_digest, self.input, self.output)
+
+    def aet(self, backend=None):
+        """the AET as a dict with tvm_aet's (and oracle.tracegen.aet_arrays's) keys; the three hash traces are expanded on
+        `backend`'s device, and are None without a backend"""
+        a = AetStruct()
+        if backend is not None:
+            backend._chk(self._l.tvm_execution_aet(backend._h, self._h, ctypes.byref(a)))
+        else:
+            _check_plain(self._l.tvm_execution_aet(None, self._h, ctypes.byref(a)))
+        d = dict(program=_rows(a.program, a.program_len, 0),
+                 instruction_multiplicities=_rows(a.instruction_multiplicities, a.program_len, 0, np.uint32),
+                 lookup_table_lookup_multiplicities=_rows(a.lookup_table_lookup_multiplicities, 256, 0))
+        for name, width in _AET_WIDTHS.items():
+            count = getattr(a, _AET_COUNTS[name])
+            ptr = getattr(a, name)
+            d[name] = _rows(ptr, count, width) if (ptr or not count) else None
+        return d
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._l.tvm_execution_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def _check_plain(rc, msg=""):
+    if rc:
+        raise TvmError(rc, lib().tvm_strerror(rc).decode() + (" | " + msg if msg else ""))
+
+
+def trace_execution(words, public_input=(), secret_input=(), digests=(), ram=None):
+    """VM::trace_execution on the host (no GPU): program words (Program::to_bwords()), public input, NonDeterminism (secret
+    input, digests [k][5], initial RAM {address: value}) -> Execution.  A program the VM rejects raises TvmError with code
+    TVM_ERR_VM (-10) and the reference's error variant in the message."""
+    w, wp = _np_u64(np.array(list(words), dtype=np.uint64))
+    i, ip = _np_u64(np.array(list(public_input), dtype=np.uint64))
+    sec, sp = _np_u64(np.array(list(secret_input), dtype=np.uint64))
+    dg, dp = _np_u64(np.array([list(d) for d in digests], dtype=np.uint64).reshape(-1, 5))
+    ram = dict(ram or {})
+    ra, rap = _np_u64(np.array(list(ram.keys()), dtype=np.uint64))
+    rv, rvp = _np_u64(np.array(list(ram.values()), dtype=np.uint64))
+    nd = NondeterminismStruct(sp, sec.size, dp, dg.shape[0], rap, rvp, ra.size)
+    h = _vp()
+    msg = ctypes.create_string_buffer(512)
+    rc = lib().tvm_trace_execution(wp, w.size, ip, i.size, ctypes.byref(nd), ctypes.byref(h), msg, 512)
+    _check_plain(rc, msg.value.decode())
+    return Execution(h, [int(v) for v in i])
 
 
 def derive_domains(security_level=160, log2_expansion=2, padded_height=1 << 10, ldt_choice=LDT_AUTO, conjectured=False):
@@ -726,6 +830,31 @@ class Backend:
         del keep, keep_claim
         self._chk(rc)
         return buf[:cap.value].copy()
+
+    def prove_execution(self, ex, seed, security_level=160, log2_expansion=2, ldt_choice=LDT_AUTO, conjectured=False):
+        """tvm_prove_execution: Stark::prove of an Execution's claim from its AET (hash traces expanded on the device) and the
+        prover's 32-byte randomness seed -> proof words.  The seed must come from a CSPRNG the verifier cannot predict."""
+        dom = derive_domains(security_level, log2_expansion, ex.padded_height, ldt_choice, conjectured)
+        p = Params(security_level, log2_expansion, ldt_choice, int(conjectured))
+        est = _proof_capacity(dom)
+        for _ in range(2):
+            buf = np.empty(est, dtype=np.uint64)
+            cap = ctypes.c_size_t(est)
+            rc = self._l.tvm_prove_execution(self._h, ctypes.byref(p), ex._h, self._seed(seed), buf.ctypes.data_as(_u64p), ctypes.byref(cap))
+            if rc == -1 and cap.value > est:    # the proof is longer than the estimate: prove again into a buffer that fits
+                est = cap.value
+                continue
+            break
+        self._chk(rc)
+        return buf[:cap.value].copy()
+
+    def prove_program(self, words, public_input=(), secret_input=(), digests=(), ram=None, seed=None, **params):
+        """triton_vm::prove_program (lib.rs:228-267): trace the program on the host, prove on this GPU -> (claim, proof)"""
+        ex = trace_execution(words, public_input, secret_input, digests, ram)
+        try:
+            return ex.claim, self.prove_execution(ex, seed, **params)
+        finally:
+            ex.close()
 
     def prove_tables_seeded(self, claim, main_table, seed, security_level=160, log2_expansion=2, padded_height=None, ldt_choice=LDT_AUTO,
                             conjectured=False, fill_derived_main_columns=True):
