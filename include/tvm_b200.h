@@ -396,6 +396,55 @@ int tvm_aux_extend(tvm_ctx *ctx, const uint64_t *main_trace, unsigned log2_n, co
  * degree-lowering columns 149..378 of main_trace [379][n] (canonical, column-major, host or device memory, IN PLACE) from
  * the 149 table columns 0..148, which are not modified. */
 int tvm_fill_derived_main_columns(tvm_ctx *ctx, uint64_t *main_trace, unsigned log2_n);
+/* ---- AIR constraint check of a witness: the reference's test-suite check check_constraints_fn! (stark.rs:2899-3015) on the
+ *      device, for the degree-lowered AIR the prover enforces.  A witness that violates a constraint still gives a proof, which
+ *      tvm_verify then rejects without saying where; these entry points name every violated constraint, its origin and rows.
+ *      All 604 constraints are checked in evaluator order (init | cons | tran | term, base-field-valued before
+ *      extension-field-valued; the order of tvm_air_quotient_dev's weights): init on row 0, cons on every row, tran on the pairs
+ *      (i, i+1) for i < n - 1 (no wrap-around), term on row n - 1.
+ *      Outputs, per constraint j: counts[j] rows where its value is non-zero, first_rows[j] / last_rows[j] the first and last
+ *      such row (UINT64_MAX when counts[j] == 0); *num_violated the number of constraints with counts[j] != 0.  Violations are
+ *      results: the call returns TVM_OK whenever the check ran.  The result does not depend on the launch order.
+ *
+ *      tvm_air_check: main_table [379][n] and aux_table [91][n][3] canonical, column-major (the tvm_aux_extend layout, host or
+ *      device memory; aux column 90 is read by no constraint); challenges [63][3] canonical (host), the order tvm_aux_extend
+ *      takes them; n = 2^log2_n, log2_n <= 26 (else TVM_ERR_DOMAIN).  NULL pointers are TVM_ERR_INVALID_ARG before any
+ *      kernel is launched.  A word >= p is TVM_ERR_INVALID_ARG too, found by the upload pass that converts the tables (no
+ *      check kernel runs); tvm_last_error names the table, column and row of the first one. */
+int tvm_air_check(tvm_ctx *ctx, const uint64_t *main_table, const uint64_t *aux_table, unsigned log2_n, const uint64_t *challenges,
+                  uint64_t *counts, uint64_t *first_rows, uint64_t *last_rows, uint64_t *num_violated);
+/*      tvm_air_check_aet: the witness as tvm_prove_aet builds it, checked without leaving the device: MasterMainTable::new +
+ *      pad from the AET (num_rows as tvm_main_table_from_aet takes it), the degree-lowering columns, Challenges::new (the 4
+ *      challenges derived from `claim` and the lookup table, challenges.rs:88-135) on top of sampled_challenges [59][3]
+ *      (canonical), MasterMainTable::extend with a zero randomizer column, then the check.
+ *      tvm_air_check_execution: the same for an execution (tvm_trace_execution): its claim and padded height, the hash traces
+ *      expanded on the device as tvm_prove_execution does.  A valid witness satisfies the AIR for every challenge value. */
+int tvm_air_check_aet(tvm_ctx *ctx, const tvm_aet *aet, const tvm_claim *claim, uint64_t num_rows, const uint64_t *sampled_challenges,
+                      uint64_t *counts, uint64_t *first_rows, uint64_t *last_rows, uint64_t *num_violated);
+int tvm_air_check_execution(tvm_ctx *ctx, const tvm_execution *ex, const uint64_t *sampled_challenges, uint64_t *counts,
+                            uint64_t *first_rows, uint64_t *last_rows, uint64_t *num_violated);
+/*      tvm_air_constraint_info (host code, no GPU): constraint `index` < 604 of the evaluator order.
+ *        origin        0..8 the table, in the order of tvm_main_table_from_aet's table_lengths_out; 9 the Grand Cross-Table
+ *                      Argument; 10 degree lowering (a substitution constraint, which defines a derived column)
+ *        origin_index  an original constraint's position in its table's list for that category before degree lowering (the
+ *                      idx of the reference's ConstraintError); for a substitution constraint the derived column it defines
+ *        derived_column TVM_AIR_DERIVED_MAIN (origin_index is a main column 149..378), TVM_AIR_DERIVED_AUX (an aux column
+ *                      49..89) or TVM_AIR_DERIVED_NONE
+ *        degree        the constraint's degree (the reference's generated quotient degree bounds)
+ *        origin_name   static string: "ProcessorTable", ..., "GrandCrossTableArg", "DegreeLowering" */
+#define TVM_AIR_DERIVED_NONE 0
+#define TVM_AIR_DERIVED_MAIN 1
+#define TVM_AIR_DERIVED_AUX 2
+typedef struct tvm_air_constraint {
+  uint32_t category;            /* 0 initial, 1 consistency, 2 transition, 3 terminal */
+  uint32_t index_in_category;
+  uint32_t degree;
+  uint32_t origin;
+  uint32_t origin_index;
+  uint32_t derived_column;
+  const char *origin_name;
+} tvm_air_constraint;
+int tvm_air_constraint_info(unsigned index, tvm_air_constraint *out);
 /* ---- Stark::verify (stark.rs:1388-1763, Verifier::verify) — SURVEY.md 8(f).4.
  *      Replays the Fiat-Shamir transcript of `proof` (Proof.0, canonical words) against `claim` under `params`: AIR / quotient
  *      identity at the out-of-domain point, FRI or STIR, Merkle openings, DEEP combination.  Host code — one proof is a few

@@ -767,6 +767,82 @@ int tvm_prove_execution(tvm_ctx *ctx, const tvm_params *params, const tvm_execut
 
 void tvm_execution_destroy(tvm_execution *ex) { delete ex; }
 
+int tvm_air_check(tvm_ctx *ctx, const uint64_t *main_table, const uint64_t *aux_table, unsigned log2_n, const uint64_t *challenges,
+                  uint64_t *counts, uint64_t *first_rows, uint64_t *last_rows, uint64_t *num_violated) {
+  if (!ctx || !main_table || !aux_table || !challenges || !counts || !first_rows || !last_rows || !num_violated) return TVM_ERR_INVALID_ARG;
+  if (log2_n > 26) return TVM_ERR_DOMAIN;
+  TVM_API_BEGIN(ctx)
+  for (size_t i = 0; i < 3 * TVM_NUM_CHALLENGES; i++)
+    if (challenges[i] >= P) throw ApiError{TVM_ERR_INVALID_ARG, "challenge word >= p at index " + std::to_string(i)};
+  Ctx &c = *c__;
+  const size_t n = (size_t)1 << log2_n;
+  std::vector<u64> ch_mont(3 * TVM_NUM_CHALLENGES);
+  for (size_t i = 0; i < ch_mont.size(); i++) ch_mont[i] = to_mont(challenges[i]);
+  DevMem mem(c);
+  u64 *d_main, *d_aux;
+  air_check_upload(c, mem, (const u64 *)main_table, (const u64 *)aux_table, n, &d_main, &d_aux);
+  air_check_run(c, mem, d_main, d_aux, n, ch_mont.data(), counts, first_rows, last_rows, num_violated);
+  TVM_API_END
+}
+
+// the witness tvm_prove_aet builds (fill, padding, degree-lowering columns, Challenges::new, extend with a zero randomizer
+// column), checked in place
+static void air_check_witness(Ctx &c, DevMem &mem, const tvm_aet &aet, const ClaimView &cv, size_t n, const uint64_t *sampled,
+                              uint64_t *counts, uint64_t *first_rows, uint64_t *last_rows, uint64_t *num_violated) {
+  const size_t NM = TVM_NUM_MAIN_COLUMNS, NB = TVM_NUM_MAIN_TABLE_COLUMNS, NA = TVM_NUM_AUX_COLUMNS;
+  std::vector<xfe> ch;
+  for (int i = 0; i < 59; i++) ch.push_back(xmake(to_mont(sampled[3 * i]), to_mont(sampled[3 * i + 1]), to_mont(sampled[3 * i + 2])));
+  challenges_derive(cv, ch);
+  std::vector<u64> ch_mont;
+  for (xfe x : ch) { ch_mont.push_back(x.c0); ch_mont.push_back(x.c1); ch_mont.push_back(x.c2); }
+  u64 *d_main = mem.words(NM * n);
+  {
+    DevMem fill_mem(c);
+    main_fill_run(c, fill_mem, aet, n, d_main, nullptr);
+  }
+  to_mont_run(c, d_main, NB * n);
+  main_derived_run(c, d_main, n);
+  u64 *d_aux = mem.words(3 * NA * n);
+  u64 *d_misc = mem.words(3 * TVM_NUM_CHALLENGES + aux_extend_scratch_words(n));
+  TVM_CUDA(cudaMemcpyAsync(d_misc, ch_mont.data(), 3 * TVM_NUM_CHALLENGES * 8, cudaMemcpyHostToDevice, c.stream));
+  TVM_CUDA(cudaMemsetAsync(d_aux + 3 * (NA - 1) * n, 0, 3 * n * 8, c.stream));
+  aux_extend_run(c, d_main, n, d_misc, d_aux, d_misc + 3 * TVM_NUM_CHALLENGES);
+  mem.release(d_misc);
+  air_check_run(c, mem, d_main, d_aux, n, ch_mont.data(), counts, first_rows, last_rows, num_violated);
+}
+
+static bool canonical_words(const uint64_t *w, size_t n) {
+  for (size_t i = 0; i < n; i++) if (w[i] >= P) return false;
+  return true;
+}
+
+int tvm_air_check_aet(tvm_ctx *ctx, const tvm_aet *aet, const tvm_claim *claim, uint64_t num_rows, const uint64_t *sampled_challenges,
+                      uint64_t *counts, uint64_t *first_rows, uint64_t *last_rows, uint64_t *num_violated) {
+  if (!ctx || !aet || !claim || !sampled_challenges || !counts || !first_rows || !last_rows || !num_violated) return TVM_ERR_INVALID_ARG;
+  if (!claim_ok(claim) || !canonical_words(sampled_challenges, 3 * 59)) return TVM_ERR_INVALID_ARG;
+  if (num_rows < 256 || (num_rows & (num_rows - 1)) || num_rows > ((uint64_t)1 << 26)) return TVM_ERR_DOMAIN;
+  TVM_API_BEGIN(ctx)
+  const ClaimView cv{claim->program_digest, claim->version, claim->input, claim->num_input, claim->output, claim->num_output};
+  DevMem mem(*c__);
+  air_check_witness(*c__, mem, *aet, cv, (size_t)num_rows, sampled_challenges, counts, first_rows, last_rows, num_violated);
+  TVM_API_END
+}
+
+int tvm_air_check_execution(tvm_ctx *ctx, const tvm_execution *ex, const uint64_t *sampled_challenges, uint64_t *counts,
+                            uint64_t *first_rows, uint64_t *last_rows, uint64_t *num_violated) {
+  if (!ctx || !ex || !sampled_challenges || !counts || !first_rows || !last_rows || !num_violated) return TVM_ERR_INVALID_ARG;
+  if (!canonical_words(sampled_challenges, 3 * 59)) return TVM_ERR_INVALID_ARG;
+  TVM_API_BEGIN(ctx)
+  const ClaimView cv{ex->digest, TVM_CURRENT_VERSION, ex->input.data(), ex->input.size(), ex->output.data(), ex->output.size()};
+  DevMem mem(*c__);
+  tvm_aet a = execution_aet_host(*ex);
+  u64 *d[3];
+  hash_trace_run(*c__, mem, *ex, d);
+  a.program_hash_trace = d[0]; a.sponge_trace = d[1]; a.hash_trace = d[2];
+  air_check_witness(*c__, mem, a, cv, ex->padded_height, sampled_challenges, counts, first_rows, last_rows, num_violated);
+  TVM_API_END
+}
+
 int tvm_bezout_coefficients(tvm_ctx *ctx, const uint64_t *roots, uint64_t m, uint64_t *a_out, uint64_t *b_out) {
   if (!ctx || (m && (!roots || !a_out || !b_out))) return TVM_ERR_INVALID_ARG;
   if (m > ((uint64_t)1 << 24)) return TVM_ERR_DOMAIN;

@@ -186,6 +186,16 @@ void evaluate_cols(Ctx &c, const u64 *d_coef, size_t coef_stride, unsigned fold_
 
 }  // namespace
 
+void challenges_derive(const ClaimView &claim, std::vector<xfe> &ch) {
+  u64 lut[256];
+  for (int i = 0; i < 256; i++) lut[i] = TIP5_LOOKUP_HOST[i];
+  xfe compressed_digest = eval_arg_terminal(claim.program_digest, 5, ch[0]);
+  xfe input_terminal = eval_arg_terminal(claim.input, claim.num_input, ch[1]);
+  xfe output_terminal = eval_arg_terminal(claim.output, claim.num_output, ch[2]);
+  xfe lookup_terminal = eval_arg_terminal(lut, 256, ch[54]);
+  ch.push_back(input_terminal); ch.push_back(output_terminal); ch.push_back(lookup_terminal); ch.push_back(compressed_digest);
+}
+
 void stark_prove(Ctx &c, const StarkParams &sp, const ClaimView &claim, size_t padded_height, const u64 *h_main_trace,
                  const u64 *h_main_rand, AuxCallback aux_cb, void *aux_user, const u64 *h_quot_rand, std::vector<u64> &proof,
                  ProveTimings *timings, const DeviceTables *dev_tables, const ExternalTranscript *ext) {
@@ -436,15 +446,7 @@ void stark_prove(Ctx &c, const StarkParams &sp, const ClaimView &claim, size_t p
 
   // ---- challenges (stark.rs:374-376, challenges.rs:88-135) -------------------------------------------
   std::vector<xfe> ch = ps.sample_scalars(59);
-  {
-    u64 lut[256];
-    for (int i = 0; i < 256; i++) lut[i] = TIP5_LOOKUP_HOST[i];
-    xfe compressed_digest = eval_arg_terminal(claim.program_digest, 5, ch[0]);
-    xfe input_terminal = eval_arg_terminal(claim.input, claim.num_input, ch[1]);
-    xfe output_terminal = eval_arg_terminal(claim.output, claim.num_output, ch[2]);
-    xfe lookup_terminal = eval_arg_terminal(lut, 256, ch[54]);
-    ch.push_back(input_terminal); ch.push_back(output_terminal); ch.push_back(lookup_terminal); ch.push_back(compressed_digest);
-  }
+  challenges_derive(claim, ch);
   std::vector<u64> ch_canon, ch_mont;
   for (xfe x : ch) {
     push_xfe_canon(ch_canon, x);

@@ -52,6 +52,9 @@ struct ClaimView {            // proof.rs:68-88, canonical words
   const u64 *input; size_t num_input;
   const u64 *output; size_t num_output;
 };
+// Challenges::new (challenges.rs:88-135): appends the 4 challenges derived from the claim and the lookup table to the 59
+// sampled ones (Montgomery form), which gives the 63 in the order the AIR reads them
+void challenges_derive(const ClaimView &claim, std::vector<xfe> &ch);
 // Given the 63 challenges (canonical), provides aux_trace [91][n][3] and aux_rand [91][h][3] (canonical).
 // The callee sets *aux_trace / *aux_rand to its own (ideally pinned) buffers, which must stay valid
 // until prove returns (zero copy: the library reads them straight into the H2D transfer).
@@ -81,6 +84,15 @@ void main_fill_run(Ctx &c, struct DevMem &mem, const tvm_aet &aet, size_t n, u64
 void bezout_run(Ctx &c, struct DevMem &mem, const u64 *d_roots_mont, size_t m, u64 *d_a, u64 *d_b);
 // the three hash traces of an execution (fill/hash_trace.cuh) into device memory of `mem`: d_out[section] [rows][67] canonical
 void hash_trace_run(Ctx &c, struct DevMem &mem, const tvm_execution &ex, u64 *d_out[3]);
+
+// ---- air_check.cu: every AIR constraint on the rows where it must vanish (check_constraints_fn!, stark.rs:2899-3015) ----
+// main [379][n] and aux [91][n][3] canonical, host or device memory -> Montgomery device copies in `mem`: main [379][n] and
+// the aux planes [270][n] (column 90 is read by no constraint).  A word >= p is an ApiError naming its column and row.
+void air_check_upload(Ctx &c, struct DevMem &mem, const u64 *main, const u64 *aux, size_t n, u64 **d_main, u64 **d_aux);
+// d_main [379][n], d_aux planes [>= 270][n] (Montgomery, device); ch_mont the 63 challenges (host, Montgomery X-field).
+// counts / first / last [604] (host): violating rows per constraint; first = last = UINT64_MAX when there are none.
+void air_check_run(Ctx &c, struct DevMem &mem, const u64 *d_main, const u64 *d_aux, size_t n, const u64 *ch_mont, uint64_t *counts,
+                   uint64_t *first, uint64_t *last, uint64_t *num_violated);
 
 // ---- prover_randomness.cu: the prover's four randomness arrays from its 32-byte seed, CANONICAL, concatenated ----
 struct ProverRandomnessLayout {   // word offsets into the concatenation, and its length

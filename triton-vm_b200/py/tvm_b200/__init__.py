@@ -8,6 +8,7 @@ raises `TvmError`.
 import ctypes
 import os
 import subprocess
+import sys
 import numpy as np
 
 _PKG = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))  # triton-vm_b200/
@@ -26,7 +27,7 @@ class TvmError(RuntimeError):
 
 def build(force=False, verbose=False):
     """Compile libtvm_b200.so for sm_90a in-tree (nvcc cross-compiles without a GPU)."""
-    args = ["make", "-C", _PKG, "-j8", "lib/libtvm_b200.so"]
+    args = ["make", "-C", _PKG, "-j8", "PYTHON=" + sys.executable, "lib/libtvm_b200.so"]   # the generators run on this interpreter
     if force:
         args.insert(1, "-B")
     r = subprocess.run(args, capture_output=True, text=True)
@@ -147,6 +148,14 @@ class CommStruct(ctypes.Structure):   # tvm_comm
 
 LDT_AUTO, LDT_FRI, LDT_STIR = 0, 1, 2      # tvm_params.ldt_choice
 
+
+class AirConstraintStruct(ctypes.Structure):   # tvm_air_constraint
+    _fields_ = [(n, ctypes.c_uint32) for n in ("category", "index_in_category", "degree", "origin", "origin_index", "derived_column")] + \
+        [("origin_name", ctypes.c_char_p)]
+
+
+_U64x604 = ctypes.c_uint64 * 604
+
 _lib = None
 NUM_MAIN_COLUMNS, NUM_AUX_COLUMNS, NUM_CHALLENGES = 379, 91, 63      # include/tvm_b200.h
 
@@ -218,6 +227,11 @@ _SIGNATURES = {
     "tvm_execution_destroy": (None, [_vp]),
     "tvm_air_quotient_dev": (ctypes.c_int, [_vp, _vp, ctypes.c_size_t, _vp, ctypes.c_size_t, _u64p, _u64p, ctypes.c_uint,
                                             ctypes.c_uint, ctypes.c_uint64, _vp, ctypes.c_size_t]),
+    "tvm_air_check": (ctypes.c_int, [_vp, _u64p, _u64p, ctypes.c_uint, _u64p, _u64p, _u64p, _u64p, _u64p]),
+    "tvm_air_check_aet": (ctypes.c_int, [_vp, ctypes.POINTER(AetStruct), ctypes.POINTER(ClaimStruct), ctypes.c_uint64, _u64p, _u64p, _u64p,
+                                         _u64p, _u64p]),
+    "tvm_air_check_execution": (ctypes.c_int, [_vp, _vp, _u64p, _u64p, _u64p, _u64p, _u64p]),
+    "tvm_air_constraint_info": (ctypes.c_int, [ctypes.c_uint, ctypes.POINTER(AirConstraintStruct)]),
 }
 
 
@@ -398,6 +412,39 @@ def trace_execution(words, public_input=(), secret_input=(), digests=(), ram=Non
     rc = lib().tvm_trace_execution(wp, w.size, ip, i.size, ctypes.byref(nd), ctypes.byref(h), msg, 512)
     _check_plain(rc, msg.value.decode())
     return Execution(h, [int(v) for v in i])
+
+
+AIR_CATEGORIES = ("init", "cons", "tran", "term")
+NUM_CONSTRAINTS = 604
+_AIR_INFO = None
+
+
+def air_constraint_info():
+    """tvm_air_constraint_info for all 604 constraints of the evaluator order (host code, no GPU) -> list of dicts: index,
+    category ("init" | "cons" | "tran" | "term"), index_in_category, degree, origin (the table's name, "GrandCrossTableArg"
+    or "DegreeLowering"), origin_id (0..8 the tables in TABLES order, 9, 10), origin_index (an original constraint's position
+    in its table's list before degree lowering; a substitution constraint's derived column) and derived_column (None, or
+    ("main", column) / ("aux", column) for a substitution constraint)"""
+    global _AIR_INFO
+    if _AIR_INFO is None:
+        out = []
+        for j in range(NUM_CONSTRAINTS):
+            c = AirConstraintStruct()
+            _check_plain(lib().tvm_air_constraint_info(j, ctypes.byref(c)))
+            out.append(dict(index=j, category=AIR_CATEGORIES[c.category], index_in_category=int(c.index_in_category), degree=int(c.degree),
+                            origin=c.origin_name.decode(), origin_id=int(c.origin), origin_index=int(c.origin_index),
+                            derived_column=(None, ("main", int(c.origin_index)), ("aux", int(c.origin_index)))[c.derived_column]))
+        _AIR_INFO = out
+    return [dict(d) for d in _AIR_INFO]
+
+
+def _air_check_result(counts, first, last, arrays):
+    """the outputs of a tvm_air_check* call -> (counts, first_rows, last_rows) numpy arrays, or the list of violated constraints"""
+    c, f, l = (np.ctypeslib.as_array(x).copy() for x in (counts, first, last))
+    if arrays:
+        return c, f, l
+    info = air_constraint_info()
+    return [dict(info[j], count=int(c[j]), first_row=int(f[j]), last_row=int(l[j])) for j in np.nonzero(c)[0]]
 
 
 def derive_domains(security_level=160, log2_expansion=2, padded_height=1 << 10, ldt_choice=LDT_AUTO, conjectured=False):
@@ -853,6 +900,56 @@ class Backend:
         ex = trace_execution(words, public_input, secret_input, digests, ram)
         try:
             return ex.claim, self.prove_execution(ex, seed, **params)
+        finally:
+            ex.close()
+
+    # ---- AIR constraint check (tvm_air_check*) -------------------------------------------
+    def air_check(self, main, aux, challenges, arrays=False):
+        """tvm_air_check: every AIR constraint on the rows where it must vanish.  main [379, n], aux [91, n, 3] canonical (numpy,
+        or contiguous torch tensors on the host or this GPU), challenges [63, 3] canonical -> the violated constraints (dicts of
+        air_constraint_info() plus count, first_row, last_row), or with arrays=True (counts, first_rows, last_rows) [604] each"""
+        km, mp, mshape = _u64_arg(main)
+        ka, ap, ashape = _u64_arg(aux)
+        assert len(mshape) == 2 and mshape[0] == NUM_MAIN_COLUMNS, mshape
+        n = mshape[1]
+        assert int(np.prod(ashape)) == NUM_AUX_COLUMNS * n * 3, ashape
+        ch, chp = _np_u64(np.asarray(challenges, dtype=np.uint64).reshape(NUM_CHALLENGES, 3))
+        out = [_U64x604() for _ in range(3)]
+        nv = ctypes.c_uint64()
+        self._chk(self._l.tvm_air_check(self._h, mp, ap, max(n.bit_length() - 1, 0), chp, *out, ctypes.byref(nv)))
+        del km, ka
+        return _air_check_result(*out, arrays)
+
+    def air_check_aet(self, aet, claim, num_rows, sampled, arrays=False):
+        """tvm_air_check_aet: the witness tvm_prove_aet builds from `aet` (fill, padding to num_rows, degree-lowering columns,
+        Challenges::new from `claim` on the 59 sampled challenges [59, 3], extension) checked on the device; result as air_check"""
+        s, keep = aet_struct(aet)
+        cs, keep_claim = self._claim(claim)
+        sp_, spp = _np_u64(np.asarray(sampled, dtype=np.uint64).reshape(59, 3))
+        out = [_U64x604() for _ in range(3)]
+        nv = ctypes.c_uint64()
+        rc = self._l.tvm_air_check_aet(self._h, ctypes.byref(s), ctypes.byref(cs), int(num_rows), spp, *out, ctypes.byref(nv))
+        del keep, keep_claim
+        self._chk(rc)
+        return _air_check_result(*out, arrays)
+
+    def air_check_execution(self, ex, sampled, arrays=False):
+        """tvm_air_check_execution: an Execution's witness at its padded height, checked on the device; result as air_check"""
+        sp_, spp = _np_u64(np.asarray(sampled, dtype=np.uint64).reshape(59, 3))
+        out = [_U64x604() for _ in range(3)]
+        nv = ctypes.c_uint64()
+        self._chk(self._l.tvm_air_check_execution(self._h, ex._h, spp, *out, ctypes.byref(nv)))
+        return _air_check_result(*out, arrays)
+
+    def check_program(self, words, public_input=(), secret_input=(), digests=(), ram=None, sampled=None, arrays=False):
+        """trace the program on the host and check its witness against every AIR constraint on this GPU -> as air_check.
+        `sampled`: the 59 sampled challenges [59, 3]; by default drawn with numpy from a fixed seed (a valid witness satisfies
+        the AIR for every challenge value; the library draws no entropy)."""
+        if sampled is None:
+            sampled = np.random.default_rng(0x7A1C).integers(0, P, size=(59, 3), dtype=np.uint64)
+        ex = trace_execution(words, public_input, secret_input, digests, ram)
+        try:
+            return self.air_check_execution(ex, sampled, arrays)
         finally:
             ex.close()
 
