@@ -133,16 +133,6 @@ void lde_run(Ctx &c, const u64 *d_trace, const u64 *d_rand, unsigned num_rand, u
     return translate_exception(c__); \
   }
 
-// proof.rs:68-88: a claim's words are field elements; NULL with a non-zero count or a word >= p is an argument error (a
-// non-canonical word would otherwise alias the claim [x] with [x + p] in the transcript)
-static bool claim_ok(const tvm_claim *c) {
-  if ((c->num_input && !c->input) || (c->num_output && !c->output)) return false;
-  for (int i = 0; i < 5; i++) if (c->program_digest[i] >= tvm::P) return false;
-  for (size_t i = 0; i < c->num_input; i++) if (c->input[i] >= tvm::P) return false;
-  for (size_t i = 0; i < c->num_output; i++) if (c->output[i] >= tvm::P) return false;
-  return true;
-}
-
 // the prover's randomness for `seed` in device memory of `mem` (canonical; main, aux, column 90, quotient segments)
 struct SeededRandomness {
   const u64 *main_rand, *aux_rand, *randomizer_column, *quot_rand;
@@ -156,6 +146,44 @@ static SeededRandomness seeded_randomness(Ctx &c, DevMem &mem, const StarkParams
   prover_randomness_run(c, seed, d.trace_len, d.num_trace_randomizers, d.num_quotient_randomizer_coefficients, d_r);
   return {d_r + L.main, d_r + L.aux, d_r + L.randomizer_column, d_r + L.quot, d.trace_len, d.num_trace_randomizers,
           d.num_quotient_randomizer_coefficients};
+}
+
+// the proof into the caller's buffer; *proof_len receives the proof's length even when the buffer is missing or too small,
+// so that the caller can size a second attempt
+static void copy_proof_out(const std::vector<u64> &proof, uint64_t *proof_out, size_t *proof_len) {
+  const size_t cap = *proof_len;
+  *proof_len = proof.size();
+  if (!proof_out || cap < proof.size()) throw ApiError{TVM_ERR_INVALID_ARG, "proof buffer too small"};
+  memcpy(proof_out, proof.data(), proof.size() * 8);
+}
+
+// a low-degree test's revealed indices: *num_indices (optional) receives their count, indices_out (optional) the indices
+static void copy_indices_out(const std::vector<uint32_t> &revealed, uint32_t *indices_out, size_t *num_indices) {
+  const size_t cap = num_indices ? *num_indices : 0;
+  if (num_indices) *num_indices = revealed.size();
+  if (indices_out) {
+    if (cap < revealed.size()) throw ApiError{TVM_ERR_INVALID_ARG, "index buffer too small"};
+    memcpy(indices_out, revealed.data(), revealed.size() * sizeof(uint32_t));
+  }
+}
+
+// What every tvm_prove* entry point does after its own argument checks.  With a seed the randomness is drawn into device
+// memory first (after whatever the caller already holds there, so before the prove reads free memory to choose its mode).
+// Then the prove, and the proof copied out, unless proof_len is NULL: an external transcript keeps the proof stream.
+static void run_prove(tvm_ctx *ctx, const tvm_params &params, const ClaimView &cv, uint64_t padded_height, ProveInputs in,
+                      const uint8_t *seed, uint64_t *proof_out, size_t *proof_len) {
+  Ctx &c = ctx->c;
+  const StarkParams sp = stark_params(params);
+  std::vector<u64> proof;
+  {
+    DevMem mem(c);
+    if (seed) {
+      const SeededRandomness r = seeded_randomness(c, mem, sp, padded_height, seed);
+      in.main_rand = r.main_rand; in.aux_rand = r.aux_rand; in.randomizer_column = r.randomizer_column; in.quot_rand = r.quot_rand;
+    }
+    stark_prove(c, sp, cv, padded_height, in, proof, &ctx->timings);
+  }
+  if (proof_len) copy_proof_out(proof, proof_out, proof_len);
 }
 
 extern "C" {
@@ -420,7 +448,7 @@ int tvm_air_quotient_dev(tvm_ctx *ctx, const uint64_t *d_main, size_t main_strid
 int tvm_derive_domains(const tvm_params *p, uint64_t padded_height, tvm_domains *out) {
   if (!p || !out) return TVM_ERR_INVALID_ARG;
   StarkDerived d{};
-  int rc = stark_derive(StarkParams{p->security_level, p->log2_ldt_expansion_factor, p->ldt_choice, p->soundness}, padded_height, d);
+  int rc = stark_derive(stark_params(*p), padded_height, d);
   if (rc) return rc;
   out->padded_height = d.padded_height; out->num_trace_randomizers = d.num_trace_randomizers;
   out->randomized_trace_len = d.randomized_trace_len; out->trace_len = d.trace_len; out->quotient_len = d.quotient_len;
@@ -449,21 +477,12 @@ int tvm_aux_extend(tvm_ctx *ctx, const uint64_t *main_trace, unsigned log2_n, co
   u64 *d_main = mem.words(NM * n);
   u64 *d_aux = mem.words(3 * NA * n);      // planes; reused as staging for the interleaved output
   u64 *d_out = mem.words(3 * NA * n);
-  u64 *d_misc = mem.words(3 * TVM_NUM_CHALLENGES + 3 * n + aux_extend_scratch_words(n));
-  u64 *d_ch = d_misc, *d_rc = d_misc + 3 * TVM_NUM_CHALLENGES, *d_scratch = d_rc + 3 * n;
+  u64 *d_ch = mem.words(3 * TVM_NUM_CHALLENGES);
   TVM_CUDA(cudaMemcpyAsync(d_main, main_trace, NM * n * 8, cudaMemcpyDefault, c.stream));
   TVM_CUDA(cudaMemcpyAsync(d_ch, challenges, 3 * TVM_NUM_CHALLENGES * 8, cudaMemcpyDefault, c.stream));
   to_mont_run(c, d_main, NM * n);
   to_mont_run(c, d_ch, 3 * TVM_NUM_CHALLENGES);
-  u64 *d_rplanes = d_aux + 3 * (NA - 1) * n;
-  if (randomizer_column) {
-    TVM_CUDA(cudaMemcpyAsync(d_rc, randomizer_column, 3 * n * 8, cudaMemcpyDefault, c.stream));
-    to_mont_run(c, d_rc, 3 * n);
-    deinterleave3_run(c, d_rc, d_rplanes, n, 1);
-  } else {
-    TVM_CUDA(cudaMemsetAsync(d_rplanes, 0, 3 * n * 8, c.stream));
-  }
-  aux_extend_run(c, d_main, n, d_ch, d_aux, d_scratch);
+  aux_extend_on_device(c, mem, d_main, n, d_ch, (const u64 *)randomizer_column, d_aux);
   interleave3_from_mont_run(c, d_aux, d_out, n, NA);
   TVM_CUDA(cudaMemcpyAsync(aux_trace_out, d_out, 3 * NA * n * 8, cudaMemcpyDefault, c.stream));
   TVM_CUDA(cudaStreamSynchronize(c.stream));
@@ -499,14 +518,10 @@ int tvm_prove(tvm_ctx *ctx, const tvm_params *params, const tvm_claim *claim, ui
   if (!ctx || !params || !claim || !main_trace || !main_rand || !aux_cb || !quot_rand || !proof_len) return TVM_ERR_INVALID_ARG;
   if (params->ldt_choice > 2 || !claim_ok(claim)) return TVM_ERR_INVALID_ARG;
   TVM_API_BEGIN(ctx)
-  ClaimView cv{claim->program_digest, claim->version, claim->input, claim->num_input, claim->output, claim->num_output};
-  std::vector<u64> proof;
-  stark_prove(*c__, StarkParams{params->security_level, params->log2_ldt_expansion_factor, params->ldt_choice, params->soundness}, cv, padded_height, (const u64 *)main_trace,
-              (const u64 *)main_rand, (AuxCallback)aux_cb, aux_user, (const u64 *)quot_rand, proof, &ctx->timings);
-  size_t cap = *proof_len;
-  *proof_len = proof.size();
-  if (!proof_out || cap < proof.size()) throw ApiError{TVM_ERR_INVALID_ARG, "proof buffer too small"};
-  memcpy(proof_out, proof.data(), proof.size() * 8);
+  ProveInputs in;
+  in.main_trace = (const u64 *)main_trace; in.main_rand = (const u64 *)main_rand; in.quot_rand = (const u64 *)quot_rand;
+  in.aux_cb = (AuxCallback)aux_cb; in.aux_user = aux_user;
+  run_prove(ctx, *params, claim_view(*claim), padded_height, in, nullptr, proof_out, proof_len);
   TVM_API_END
 }
 
@@ -518,13 +533,13 @@ int tvm_prove_transcript(tvm_ctx *ctx, const tvm_params *params, const tvm_claim
     return TVM_ERR_INVALID_ARG;
   if (params->ldt_choice > 2 || !claim_ok(claim)) return TVM_ERR_INVALID_ARG;
   TVM_API_BEGIN(ctx)
-  ClaimView cv{claim->program_digest, claim->version, claim->input, claim->num_input, claim->output, claim->num_output};
-  std::vector<u64> unused;
   const ExternalTranscript ext{transcript->user, transcript->alter_fiat_shamir_state, transcript->enqueue, transcript->sample_scalars,
                                transcript->sample_indices};
-  stark_prove(*c__, StarkParams{params->security_level, params->log2_ldt_expansion_factor, params->ldt_choice, params->soundness}, cv, padded_height,
-              (const u64 *)main_trace, (const u64 *)main_rand, (AuxCallback)aux_cb, aux_user, (const u64 *)quot_rand, unused, &ctx->timings, nullptr,
-              &ext);
+  ProveInputs in;
+  in.main_trace = (const u64 *)main_trace; in.main_rand = (const u64 *)main_rand; in.quot_rand = (const u64 *)quot_rand;
+  in.aux_cb = (AuxCallback)aux_cb; in.aux_user = aux_user;
+  in.ext = &ext;
+  run_prove(ctx, *params, claim_view(*claim), padded_height, in, nullptr, nullptr, nullptr);
   TVM_API_END
 }
 
@@ -534,15 +549,11 @@ int tvm_prove_tables(tvm_ctx *ctx, const tvm_params *params, const tvm_claim *cl
   if (!ctx || !params || !claim || !main_table || !main_rand || !aux_rand || !quot_rand || !proof_len) return TVM_ERR_INVALID_ARG;
   if (params->ldt_choice > 2 || !claim_ok(claim)) return TVM_ERR_INVALID_ARG;
   TVM_API_BEGIN(ctx)
-  ClaimView cv{claim->program_digest, claim->version, claim->input, claim->num_input, claim->output, claim->num_output};
-  std::vector<u64> proof;
-  DeviceTables dt{(const u64 *)aux_rand, (const u64 *)randomizer_column, fill_derived_main_columns != 0};
-  stark_prove(*c__, StarkParams{params->security_level, params->log2_ldt_expansion_factor, params->ldt_choice, params->soundness}, cv, padded_height,
-              (const u64 *)main_table, (const u64 *)main_rand, nullptr, nullptr, (const u64 *)quot_rand, proof, &ctx->timings, &dt);
-  size_t cap = *proof_len;
-  *proof_len = proof.size();
-  if (!proof_out || cap < proof.size()) throw ApiError{TVM_ERR_INVALID_ARG, "proof buffer too small"};
-  memcpy(proof_out, proof.data(), proof.size() * 8);
+  ProveInputs in;
+  in.main_trace = (const u64 *)main_table; in.fill_derived_main = fill_derived_main_columns != 0;
+  in.main_rand = (const u64 *)main_rand; in.aux_rand = (const u64 *)aux_rand; in.randomizer_column = (const u64 *)randomizer_column;
+  in.quot_rand = (const u64 *)quot_rand;
+  run_prove(ctx, *params, claim_view(*claim), padded_height, in, nullptr, proof_out, proof_len);
   TVM_API_END
 }
 
@@ -551,12 +562,10 @@ int tvm_main_table_from_aet(tvm_ctx *ctx, const tvm_aet *aet, uint64_t num_rows,
   if (num_rows < 256 || (num_rows & (num_rows - 1)) || num_rows > ((uint64_t)1 << 26)) return TVM_ERR_DOMAIN;
   TVM_API_BEGIN(ctx)
   Ctx &c = *c__;
-  const size_t n = (size_t)num_rows, NM = TVM_NUM_MAIN_COLUMNS, NB = TVM_NUM_MAIN_TABLE_COLUMNS;
+  const size_t n = (size_t)num_rows, NM = TVM_NUM_MAIN_COLUMNS;
   DevMem mem(c);
   u64 *d_main = mem.words(NM * n);
-  main_fill_run(c, mem, *aet, n, d_main, table_lengths_out);
-  to_mont_run(c, d_main, NB * n);
-  main_derived_run(c, d_main, n);
+  main_table_on_device(c, d_main, n, *aet, table_lengths_out);
   from_mont_run(c, d_main, NM * n);
   TVM_CUDA(cudaMemcpyAsync(main_table_out, d_main, NM * n * 8, cudaMemcpyDefault, c.stream));
   TVM_CUDA(cudaStreamSynchronize(c.stream));
@@ -569,15 +578,11 @@ int tvm_prove_aet(tvm_ctx *ctx, const tvm_params *params, const tvm_claim *claim
   if (!ctx || !params || !claim || !aet || !main_rand || !aux_rand || !quot_rand || !proof_len) return TVM_ERR_INVALID_ARG;
   if (params->ldt_choice > 2 || !claim_ok(claim)) return TVM_ERR_INVALID_ARG;
   TVM_API_BEGIN(ctx)
-  ClaimView cv{claim->program_digest, claim->version, claim->input, claim->num_input, claim->output, claim->num_output};
-  std::vector<u64> proof;
-  DeviceTables dt{(const u64 *)aux_rand, (const u64 *)randomizer_column, true, aet};
-  stark_prove(*c__, StarkParams{params->security_level, params->log2_ldt_expansion_factor, params->ldt_choice, params->soundness}, cv, padded_height,
-              nullptr, (const u64 *)main_rand, nullptr, nullptr, (const u64 *)quot_rand, proof, &ctx->timings, &dt);
-  size_t cap = *proof_len;
-  *proof_len = proof.size();
-  if (!proof_out || cap < proof.size()) throw ApiError{TVM_ERR_INVALID_ARG, "proof buffer too small"};
-  memcpy(proof_out, proof.data(), proof.size() * 8);
+  ProveInputs in;
+  in.aet = aet;
+  in.main_rand = (const u64 *)main_rand; in.aux_rand = (const u64 *)aux_rand; in.randomizer_column = (const u64 *)randomizer_column;
+  in.quot_rand = (const u64 *)quot_rand;
+  run_prove(ctx, *params, claim_view(*claim), padded_height, in, nullptr, proof_out, proof_len);
   TVM_API_END
 }
 
@@ -586,9 +591,8 @@ int tvm_prover_randomness(tvm_ctx *ctx, const tvm_params *params, uint64_t padde
   if (!ctx || !params || !seed || params->ldt_choice > 2) return TVM_ERR_INVALID_ARG;
   TVM_API_BEGIN(ctx)
   Ctx &c = *c__;
-  const StarkParams sp{params->security_level, params->log2_ldt_expansion_factor, params->ldt_choice, params->soundness};
   DevMem mem(c);
-  const SeededRandomness r = seeded_randomness(c, mem, sp, padded_height, seed);
+  const SeededRandomness r = seeded_randomness(c, mem, stark_params(*params), padded_height, seed);
   if (main_rand_out) TVM_CUDA(cudaMemcpyAsync(main_rand_out, r.main_rand, TVM_NUM_MAIN_COLUMNS * r.h * 8, cudaMemcpyDefault, c.stream));
   if (aux_rand_out) TVM_CUDA(cudaMemcpyAsync(aux_rand_out, r.aux_rand, TVM_NUM_AUX_COLUMNS * r.h * 3 * 8, cudaMemcpyDefault, c.stream));
   if (randomizer_column_out) TVM_CUDA(cudaMemcpyAsync(randomizer_column_out, r.randomizer_column, r.n * 3 * 8, cudaMemcpyDefault, c.stream));
@@ -602,19 +606,9 @@ int tvm_prove_aet_seeded(tvm_ctx *ctx, const tvm_params *params, const tvm_claim
   if (!ctx || !params || !claim || !aet || !seed || !proof_len) return TVM_ERR_INVALID_ARG;
   if (params->ldt_choice > 2 || !claim_ok(claim)) return TVM_ERR_INVALID_ARG;
   TVM_API_BEGIN(ctx)
-  const StarkParams sp{params->security_level, params->log2_ldt_expansion_factor, params->ldt_choice, params->soundness};
-  ClaimView cv{claim->program_digest, claim->version, claim->input, claim->num_input, claim->output, claim->num_output};
-  std::vector<u64> proof;
-  {
-    DevMem mem(*c__);
-    const SeededRandomness r = seeded_randomness(*c__, mem, sp, padded_height, seed);
-    DeviceTables dt{r.aux_rand, r.randomizer_column, true, aet};
-    stark_prove(*c__, sp, cv, padded_height, nullptr, r.main_rand, nullptr, nullptr, r.quot_rand, proof, &ctx->timings, &dt);
-  }
-  size_t cap = *proof_len;
-  *proof_len = proof.size();
-  if (!proof_out || cap < proof.size()) throw ApiError{TVM_ERR_INVALID_ARG, "proof buffer too small"};
-  memcpy(proof_out, proof.data(), proof.size() * 8);
+  ProveInputs in;
+  in.aet = aet;
+  run_prove(ctx, *params, claim_view(*claim), padded_height, in, seed, proof_out, proof_len);
   TVM_API_END
 }
 
@@ -624,27 +618,10 @@ int tvm_prove_tables_seeded(tvm_ctx *ctx, const tvm_params *params, const tvm_cl
   if (!ctx || !params || !claim || !main_table || !seed || !proof_len) return TVM_ERR_INVALID_ARG;
   if (params->ldt_choice > 2 || !claim_ok(claim)) return TVM_ERR_INVALID_ARG;
   TVM_API_BEGIN(ctx)
-  const StarkParams sp{params->security_level, params->log2_ldt_expansion_factor, params->ldt_choice, params->soundness};
-  ClaimView cv{claim->program_digest, claim->version, claim->input, claim->num_input, claim->output, claim->num_output};
-  std::vector<u64> proof;
-  {
-    DevMem mem(*c__);
-    const SeededRandomness r = seeded_randomness(*c__, mem, sp, padded_height, seed);
-    DeviceTables dt{r.aux_rand, r.randomizer_column, fill_derived_main_columns != 0};
-    stark_prove(*c__, sp, cv, padded_height, (const u64 *)main_table, r.main_rand, nullptr, nullptr, r.quot_rand, proof, &ctx->timings, &dt);
-  }
-  size_t cap = *proof_len;
-  *proof_len = proof.size();
-  if (!proof_out || cap < proof.size()) throw ApiError{TVM_ERR_INVALID_ARG, "proof buffer too small"};
-  memcpy(proof_out, proof.data(), proof.size() * 8);
+  ProveInputs in;
+  in.main_trace = (const u64 *)main_table; in.fill_derived_main = fill_derived_main_columns != 0;
+  run_prove(ctx, *params, claim_view(*claim), padded_height, in, seed, proof_out, proof_len);
   TVM_API_END
-}
-
-static void set_failure(char *failure, size_t capacity, const std::string &text) {
-  if (!failure || !capacity) return;
-  const size_t n = std::min(capacity - 1, text.size());
-  memcpy(failure, text.data(), n);
-  failure[n] = 0;
 }
 
 int tvm_trace_execution(const uint64_t *program, size_t program_len, const uint64_t *public_input, size_t num_input,
@@ -679,7 +656,7 @@ int tvm_trace_execution(const uint64_t *program, size_t program_len, const uint6
     const VmInputs in{program, program_len, public_input, num_input, nd->individual_tokens, nd->num_individual_tokens,
                       nd->digests, nd->num_digests, nd->ram_addresses, nd->ram_values, nd->num_ram};
     if (int rc = trace_execution(in, *ex, why)) {
-      set_failure(failure, failure_capacity, why);
+      set_failure(failure, failure_capacity, why.c_str());
       return rc;
     }
     *out = ex.release();
@@ -715,6 +692,20 @@ static tvm_aet execution_aet_host(const tvm_execution &ex) {
   return a;
 }
 
+// the execution's AET with the three hash traces expanded into device memory of `mem`
+static tvm_aet execution_aet_device(Ctx &c, DevMem &mem, const tvm_execution &ex) {
+  tvm_aet a = execution_aet_host(ex);
+  u64 *d[3];
+  hash_trace_run(c, mem, ex, d);
+  a.program_hash_trace = d[0]; a.sponge_trace = d[1]; a.hash_trace = d[2];
+  return a;
+}
+
+// the claim an execution proves (Claim::about_program(..).with_input(..).with_output(..))
+static ClaimView execution_claim(const tvm_execution &ex) {
+  return {ex.digest, TVM_CURRENT_VERSION, ex.input.data(), ex.input.size(), ex.output.data(), ex.output.size()};
+}
+
 int tvm_execution_aet(tvm_ctx *ctx, const tvm_execution *ex, tvm_aet *out) {
   if (!ex || !out) return TVM_ERR_INVALID_ARG;
   *out = execution_aet_host(*ex);
@@ -723,8 +714,8 @@ int tvm_execution_aet(tvm_ctx *ctx, const tvm_execution *ex, tvm_aet *out) {
   Ctx &c = *c__;
   if (!ex->expanded) {
     DevMem mem(c);
-    u64 *d[3];
-    hash_trace_run(c, mem, *ex, d);
+    const tvm_aet a = execution_aet_device(c, mem, *ex);
+    const uint64_t *d[3] = {a.program_hash_trace, a.sponge_trace, a.hash_trace};
     for (int s = 0; s < 3; s++) {
       ex->hash_cache[s].resize(ex->hash_rows[s] * 67);
       if (ex->hash_rows[s])
@@ -743,25 +734,11 @@ int tvm_prove_execution(tvm_ctx *ctx, const tvm_params *params, const tvm_execut
                         size_t *proof_len) {
   if (!ctx || !params || !ex || !seed || !proof_len || params->ldt_choice > 2) return TVM_ERR_INVALID_ARG;
   TVM_API_BEGIN(ctx)
-  const StarkParams sp{params->security_level, params->log2_ldt_expansion_factor, params->ldt_choice, params->soundness};
-  StarkDerived derived{};
-  if (int rc = stark_derive(sp, ex->padded_height, derived)) throw ApiError{rc, "parameter derivation failed"};
-  const ClaimView cv{ex->digest, TVM_CURRENT_VERSION, ex->input.data(), ex->input.size(), ex->output.data(), ex->output.size()};
-  std::vector<u64> proof;
-  {
-    DevMem mem(*c__);
-    tvm_aet a = execution_aet_host(*ex);
-    u64 *d[3];
-    hash_trace_run(*c__, mem, *ex, d);
-    a.program_hash_trace = d[0]; a.sponge_trace = d[1]; a.hash_trace = d[2];
-    const SeededRandomness r = seeded_randomness(*c__, mem, sp, ex->padded_height, seed);
-    DeviceTables dt{r.aux_rand, r.randomizer_column, true, &a};
-    stark_prove(*c__, sp, cv, ex->padded_height, nullptr, r.main_rand, nullptr, nullptr, r.quot_rand, proof, &ctx->timings, &dt);
-  }
-  size_t cap = *proof_len;
-  *proof_len = proof.size();
-  if (!proof_out || cap < proof.size()) throw ApiError{TVM_ERR_INVALID_ARG, "proof buffer too small"};
-  memcpy(proof_out, proof.data(), proof.size() * 8);
+  DevMem mem(*c__);   // the hash traces, allocated before the seeded randomness and live throughout the prove
+  const tvm_aet a = execution_aet_device(*c__, mem, *ex);
+  ProveInputs in;
+  in.aet = &a;
+  run_prove(ctx, *params, execution_claim(*ex), ex->padded_height, in, seed, proof_out, proof_len);
   TVM_API_END
 }
 
@@ -786,28 +763,21 @@ int tvm_air_check(tvm_ctx *ctx, const uint64_t *main_table, const uint64_t *aux_
 }
 
 // the witness tvm_prove_aet builds (fill, padding, degree-lowering columns, Challenges::new, extend with a zero randomizer
-// column), checked in place
+// column), by the prover's own table stages, checked in place
 static void air_check_witness(Ctx &c, DevMem &mem, const tvm_aet &aet, const ClaimView &cv, size_t n, const uint64_t *sampled,
                               uint64_t *counts, uint64_t *first_rows, uint64_t *last_rows, uint64_t *num_violated) {
-  const size_t NM = TVM_NUM_MAIN_COLUMNS, NB = TVM_NUM_MAIN_TABLE_COLUMNS, NA = TVM_NUM_AUX_COLUMNS;
   std::vector<xfe> ch;
   for (int i = 0; i < 59; i++) ch.push_back(xmake(to_mont(sampled[3 * i]), to_mont(sampled[3 * i + 1]), to_mont(sampled[3 * i + 2])));
   challenges_derive(cv, ch);
   std::vector<u64> ch_mont;
   for (xfe x : ch) { ch_mont.push_back(x.c0); ch_mont.push_back(x.c1); ch_mont.push_back(x.c2); }
-  u64 *d_main = mem.words(NM * n);
-  {
-    DevMem fill_mem(c);
-    main_fill_run(c, fill_mem, aet, n, d_main, nullptr);
-  }
-  to_mont_run(c, d_main, NB * n);
-  main_derived_run(c, d_main, n);
-  u64 *d_aux = mem.words(3 * NA * n);
-  u64 *d_misc = mem.words(3 * TVM_NUM_CHALLENGES + aux_extend_scratch_words(n));
-  TVM_CUDA(cudaMemcpyAsync(d_misc, ch_mont.data(), 3 * TVM_NUM_CHALLENGES * 8, cudaMemcpyHostToDevice, c.stream));
-  TVM_CUDA(cudaMemsetAsync(d_aux + 3 * (NA - 1) * n, 0, 3 * n * 8, c.stream));
-  aux_extend_run(c, d_main, n, d_misc, d_aux, d_misc + 3 * TVM_NUM_CHALLENGES);
-  mem.release(d_misc);
+  u64 *d_main = mem.words(TVM_NUM_MAIN_COLUMNS * n);
+  main_table_on_device(c, d_main, n, aet);
+  u64 *d_aux = mem.words(3 * TVM_NUM_AUX_COLUMNS * n);
+  u64 *d_ch = mem.words(3 * TVM_NUM_CHALLENGES);
+  TVM_CUDA(cudaMemcpyAsync(d_ch, ch_mont.data(), 3 * TVM_NUM_CHALLENGES * 8, cudaMemcpyHostToDevice, c.stream));
+  aux_extend_on_device(c, mem, d_main, n, d_ch, nullptr, d_aux);
+  mem.release(d_ch);
   air_check_run(c, mem, d_main, d_aux, n, ch_mont.data(), counts, first_rows, last_rows, num_violated);
 }
 
@@ -822,9 +792,8 @@ int tvm_air_check_aet(tvm_ctx *ctx, const tvm_aet *aet, const tvm_claim *claim, 
   if (!claim_ok(claim) || !canonical_words(sampled_challenges, 3 * 59)) return TVM_ERR_INVALID_ARG;
   if (num_rows < 256 || (num_rows & (num_rows - 1)) || num_rows > ((uint64_t)1 << 26)) return TVM_ERR_DOMAIN;
   TVM_API_BEGIN(ctx)
-  const ClaimView cv{claim->program_digest, claim->version, claim->input, claim->num_input, claim->output, claim->num_output};
   DevMem mem(*c__);
-  air_check_witness(*c__, mem, *aet, cv, (size_t)num_rows, sampled_challenges, counts, first_rows, last_rows, num_violated);
+  air_check_witness(*c__, mem, *aet, claim_view(*claim), (size_t)num_rows, sampled_challenges, counts, first_rows, last_rows, num_violated);
   TVM_API_END
 }
 
@@ -833,13 +802,9 @@ int tvm_air_check_execution(tvm_ctx *ctx, const tvm_execution *ex, const uint64_
   if (!ctx || !ex || !sampled_challenges || !counts || !first_rows || !last_rows || !num_violated) return TVM_ERR_INVALID_ARG;
   if (!canonical_words(sampled_challenges, 3 * 59)) return TVM_ERR_INVALID_ARG;
   TVM_API_BEGIN(ctx)
-  const ClaimView cv{ex->digest, TVM_CURRENT_VERSION, ex->input.data(), ex->input.size(), ex->output.data(), ex->output.size()};
   DevMem mem(*c__);
-  tvm_aet a = execution_aet_host(*ex);
-  u64 *d[3];
-  hash_trace_run(*c__, mem, *ex, d);
-  a.program_hash_trace = d[0]; a.sponge_trace = d[1]; a.hash_trace = d[2];
-  air_check_witness(*c__, mem, a, cv, ex->padded_height, sampled_challenges, counts, first_rows, last_rows, num_violated);
+  const tvm_aet a = execution_aet_device(*c__, mem, *ex);
+  air_check_witness(*c__, mem, a, execution_claim(*ex), ex->padded_height, sampled_challenges, counts, first_rows, last_rows, num_violated);
   TVM_API_END
 }
 
@@ -889,16 +854,8 @@ int tvm_stir_prove(tvm_ctx *ctx, uint32_t security_level, uint32_t soundness, ui
     revealed = stir_prove_run(c, mem, ps, d_cw, len, to_mont(7), sd, d_tmp);
     proof = ps.encode();
   }
-  const size_t icap = num_indices ? *num_indices : 0;
-  if (num_indices) *num_indices = revealed.size();
-  if (indices_out) {
-    if (icap < revealed.size()) throw ApiError{TVM_ERR_INVALID_ARG, "index buffer too small"};
-    memcpy(indices_out, revealed.data(), revealed.size() * sizeof(uint32_t));
-  }
-  const size_t cap = *proof_len;
-  *proof_len = proof.size();
-  if (!proof_out || cap < proof.size()) throw ApiError{TVM_ERR_INVALID_ARG, "proof buffer too small"};
-  memcpy(proof_out, proof.data(), proof.size() * 8);
+  copy_indices_out(revealed, indices_out, num_indices);
+  copy_proof_out(proof, proof_out, proof_len);
   TVM_API_END
 }
 
@@ -941,16 +898,8 @@ int tvm_fri_prove(tvm_ctx *ctx, uint32_t security_level, uint32_t soundness, uin
     revealed = fri_prove_run(c, mem, ps, d_cw, len, to_mont(fd.domain_offset), fd, d_in /* free again: scratch */);
     proof = ps.encode();
   }
-  const size_t icap = num_indices ? *num_indices : 0;
-  if (num_indices) *num_indices = revealed.size();
-  if (indices_out) {
-    if (icap < revealed.size()) throw ApiError{TVM_ERR_INVALID_ARG, "index buffer too small"};
-    memcpy(indices_out, revealed.data(), revealed.size() * sizeof(uint32_t));
-  }
-  const size_t cap = *proof_len;
-  *proof_len = proof.size();
-  if (!proof_out || cap < proof.size()) throw ApiError{TVM_ERR_INVALID_ARG, "proof buffer too small"};
-  memcpy(proof_out, proof.data(), proof.size() * 8);
+  copy_indices_out(revealed, indices_out, num_indices);
+  copy_proof_out(proof, proof_out, proof_len);
   TVM_API_END
 }
 

@@ -276,6 +276,22 @@ void aux_extend_run(Ctx &c, const u64 *d_main, size_t n, const u64 *d_ch, u64 *d
   TVM_CUDA(cudaGetLastError());
 }
 
+void aux_extend_on_device(Ctx &c, DevMem &mem, const u64 *d_main, size_t n, const u64 *d_ch, const u64 *randomizer_column, u64 *d_aux) {
+  const size_t NA = TVM_NUM_AUX_COLUMNS;
+  u64 *d_scratch = mem.words(aux_extend_scratch_words(n) + (randomizer_column ? 3 * n : 0));
+  u64 *d_rplanes = d_aux + 3 * (NA - 1) * n;
+  if (randomizer_column) {
+    u64 *d_rc = d_scratch + aux_extend_scratch_words(n);
+    TVM_CUDA(cudaMemcpyAsync(d_rc, randomizer_column, 3 * n * 8, cudaMemcpyDefault, c.stream));
+    to_mont_run(c, d_rc, 3 * n);
+    deinterleave3_run(c, d_rc, d_rplanes, n, 1);
+  } else {
+    TVM_CUDA(cudaMemsetAsync(d_rplanes, 0, 3 * n * 8, c.stream));
+  }
+  aux_extend_run(c, d_main, n, d_ch, d_aux, d_scratch);
+  mem.release(d_scratch);
+}
+
 // d_main [379][n] Montgomery, columns 149.. overwritten
 void main_derived_run(Ctx &c, u64 *d_main, size_t n) {
   const unsigned grid = (unsigned)((n + 127) / 128);

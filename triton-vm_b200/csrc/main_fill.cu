@@ -122,6 +122,15 @@ void main_fill_run(Ctx &c, DevMem &mem, const tvm_aet &a, size_t n, u64 *d_table
   }
 }
 
+void main_table_on_device(Ctx &c, u64 *d_main, size_t n, const tvm_aet &aet, uint64_t *lengths9) {
+  {
+    DevMem fill_mem(c);   // the AET's device copy and the fill's scratch go back to the pool right after
+    main_fill_run(c, fill_mem, aet, n, d_main, lengths9);
+  }
+  to_mont_run(c, d_main, (size_t)TVM_NUM_MAIN_TABLE_COLUMNS * n);
+  main_derived_run(c, d_main, n);
+}
+
 void bezout_run(Ctx &c, DevMem &mem, const u64 *d_roots_mont, size_t m, u64 *d_a, u64 *d_b) {
   CudaExec ex{c, mem};
   fill::bezout_coefficients(ex, d_roots_mont, m, d_a, d_b);

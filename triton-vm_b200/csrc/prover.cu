@@ -196,9 +196,9 @@ void challenges_derive(const ClaimView &claim, std::vector<xfe> &ch) {
   ch.push_back(input_terminal); ch.push_back(output_terminal); ch.push_back(lookup_terminal); ch.push_back(compressed_digest);
 }
 
-void stark_prove(Ctx &c, const StarkParams &sp, const ClaimView &claim, size_t padded_height, const u64 *h_main_trace,
-                 const u64 *h_main_rand, AuxCallback aux_cb, void *aux_user, const u64 *h_quot_rand, std::vector<u64> &proof,
-                 ProveTimings *timings, const DeviceTables *dev_tables, const ExternalTranscript *ext) {
+void stark_prove(Ctx &c, const StarkParams &sp, const ClaimView &claim, size_t padded_height, const ProveInputs &in,
+                 std::vector<u64> &proof, ProveTimings *timings) {
+  const bool dev_tables = !in.aux_cb;   // device-table mode: the table stages run here, on the device
   StarkDerived d{};
   int rc = stark_derive(sp, padded_height, d);
   if (rc) throw ApiError{rc, "parameter derivation failed"};
@@ -255,7 +255,7 @@ void stark_prove(Ctx &c, const StarkParams &sp, const ClaimView &claim, size_t p
 
   DevMem mem(c);
   ProofStream ps;
-  ps.ext = ext;
+  ps.ext = in.ext;
   ps.alter_fiat_shamir_state_with(encode_claim(claim.program_digest, claim.version, claim.input, claim.num_input, claim.output,
                                                claim.num_output));
   ps.enqueue(ItemKind::Log2PaddedHeight, {(u64)ilog2(d.padded_height)});
@@ -422,22 +422,15 @@ void stark_prove(Ctx &c, const StarkParams &sp, const ClaimView &claim, size_t p
     ExtendOpts o;
     if (dev_tables) {
       o.keep_in = &d_main_trace;
-      if (dev_tables->aet) {              // MasterMainTable::new + pad on the device, then the degree-lowering columns
+      if (in.aet) {                       // MasterMainTable::new + pad on the device, then the degree-lowering columns
         o.upload_cols = 0;
-        o.after_upload = [&](u64 *d_in) {
-          {
-            DevMem fill_mem(c);             // the AET's device copy and the fill's scratch go back to the pool right after
-            main_fill_run(c, fill_mem, *dev_tables->aet, n, d_in, nullptr);
-          }
-          to_mont_run(c, d_in, (size_t)TVM_NUM_MAIN_TABLE_COLUMNS * n);
-          main_derived_run(c, d_in, n);
-        };
-      } else if (dev_tables->fill_derived_main) {
+        o.after_upload = [&](u64 *d_in) { main_table_on_device(c, d_in, n, *in.aet); };
+      } else if (in.fill_derived_main) {
         o.upload_cols = TVM_NUM_MAIN_TABLE_COLUMNS;
         o.after_upload = [&](u64 *d_in) { main_derived_run(c, d_in, n); };
       }
     }
-    extend_table(h_main_trace, h_main_rand, NM, 1, d_main_coef, d_main_lde, o);
+    extend_table(in.main_trace, in.main_rand, NM, 1, d_main_coef, d_main_lde, o);
   }
   mark();  // 1: main LDE
   u64 *d_main_nodes = mem.words(2 * N * 5);
@@ -458,31 +451,21 @@ void stark_prove(Ctx &c, const StarkParams &sp, const ClaimView &claim, size_t p
   if (dev_tables) {
     // MasterMainTable::extend on the resident main trace (aux_extend.cu); the planes feed the interpolation directly
     u64 *d_aux_planes = mem.words(NA3 * n);
-    u64 *d_misc = mem.words(3 * TVM_NUM_CHALLENGES + 3 * n + aux_extend_scratch_words(n));
-    u64 *d_ch = d_misc, *d_rc = d_misc + 3 * TVM_NUM_CHALLENGES, *d_scratch = d_rc + 3 * n;
+    u64 *d_ch = mem.words(3 * TVM_NUM_CHALLENGES);
     TVM_CUDA(cudaMemcpyAsync(d_ch, ch_mont.data(), 3 * TVM_NUM_CHALLENGES * 8, cudaMemcpyHostToDevice, c.stream));
-    u64 *d_rplanes = d_aux_planes + 3 * (NA - 1) * n;
-    if (dev_tables->randomizer_column) {
-      TVM_CUDA(cudaMemcpyAsync(d_rc, dev_tables->randomizer_column, 3 * n * 8, cudaMemcpyDefault, c.stream));
-      to_mont_run(c, d_rc, 3 * n);
-      deinterleave3_run(c, d_rc, d_rplanes, n, 1);
-    } else {
-      TVM_CUDA(cudaMemsetAsync(d_rplanes, 0, 3 * n * 8, c.stream));
-    }
-    aux_extend_run(c, d_main_trace, n, d_ch, d_aux_planes, d_scratch);
+    aux_extend_on_device(c, mem, d_main_trace, n, d_ch, in.randomizer_column, d_aux_planes);
     TVM_CUDA(cudaStreamSynchronize(c.stream));          // ch_mont is host memory of this frame
-    mem.release(d_misc);
+    mem.release(d_ch);
     mem.release(d_main_trace);
     mark();  // extend (device)
     ExtendOpts o;
     o.d_ready = d_aux_planes;
-    extend_table(nullptr, dev_tables->aux_rand, NA, 3, d_aux_coef, d_aux_lde, o);
+    extend_table(nullptr, in.aux_rand, NA, 3, d_aux_coef, d_aux_lde, o);
     mem.release(d_aux_planes);
   } else {
-    if (!aux_cb) throw ApiError{TVM_ERR_INVALID_ARG, "aux callback missing"};
     u64 *h_aux_trace = nullptr, *h_aux_rand = nullptr;   // the callee hands back pointers to its own buffers
     TVM_CUDA(cudaStreamSynchronize(c.stream));
-    if (int crc = aux_cb(aux_user, ch_canon.data(), &h_aux_trace, &h_aux_rand)) throw ApiError{TVM_ERR_INVALID_ARG, "aux callback failed: " + std::to_string(crc)};
+    if (int crc = in.aux_cb(in.aux_user, ch_canon.data(), &h_aux_trace, &h_aux_rand)) throw ApiError{TVM_ERR_INVALID_ARG, "aux callback failed: " + std::to_string(crc)};
     if (!h_aux_trace || !h_aux_rand) throw ApiError{TVM_ERR_INVALID_ARG, "aux callback returned a null buffer"};
     mark();  // extend (caller)
     extend_table(h_aux_trace, h_aux_rand, NA, 3, d_aux_coef, d_aux_lde, ExtendOpts{});
@@ -540,7 +523,7 @@ void stark_prove(Ctx &c, const StarkParams &sp, const ClaimView &claim, size_t p
   const size_t nqr = d.num_quotient_randomizer_coefficients;
   u64 *d_qr_in = mem.words(3 * nqr);
   u64 *d_qr = mem.words(3 * nqr);
-  TVM_CUDA(cudaMemcpyAsync(d_qr_in, h_quot_rand, 3 * nqr * 8, cudaMemcpyDefault, c.stream));   // host, or device (seeded proves)
+  TVM_CUDA(cudaMemcpyAsync(d_qr_in, in.quot_rand, 3 * nqr * 8, cudaMemcpyDefault, c.stream));   // host, or device (seeded proves)
   to_mont_run(c, d_qr_in, 3 * nqr);
   deinterleave3_run(c, d_qr_in, d_qr, nqr, 1);
   u64 *d_seg_coef = mem.words(15 * seg_len);
@@ -749,7 +732,7 @@ void stark_prove(Ctx &c, const StarkParams &sp, const ClaimView &claim, size_t p
   proof = ps.encode();
   if (timings) {
     TVM_CUDA(cudaStreamSynchronize(c.stream));
-    const char *names[] = {"setup", dev_tables && dev_tables->aet ? "table fill+derived columns+LDE(main)" : dev_tables && dev_tables->fill_derived_main ? "upload+derived columns+LDE(main)" : "upload+LDE(main)",
+    const char *names[] = {"setup", dev_tables && in.aet ? "table fill+derived columns+LDE(main)" : dev_tables && in.fill_derived_main ? "upload+derived columns+LDE(main)" : "upload+LDE(main)",
                            "Merkle(main)", dev_tables ? "extend(device)" : "extend(caller)", dev_tables ? "LDE(aux)" : "upload+LDE(aux)",
                            "Merkle(aux)", "quotient(AIR)", "quotient LDE", "Merkle(quot)", "OOD rows", "linear combination+DEEP",
                            "low-degree test", "open"};

@@ -1,5 +1,6 @@
 // Prover-level declarations shared by prover.cu, stark_kernels.cu and the C ABI.
 #pragma once
+#include <cstring>
 #include <string>
 #include <vector>
 #include "ctx.h"
@@ -15,6 +16,9 @@ struct StarkParams {          // stark.rs:113-145 (proven regime)
   unsigned ldt_choice;        // 0 = heuristic (stark.rs:1942-1957), 1 = FRI, 2 = STIR
   unsigned soundness;         // 0 = ProximityRegime::Proven (default), 1 = ::Conjectured
 };
+inline StarkParams stark_params(const tvm_params &p) {
+  return StarkParams{p.security_level, p.log2_ldt_expansion_factor, p.ldt_choice, p.soundness};
+}
 static constexpr int STIR_MAX_ROUNDS = 16;
 static constexpr unsigned STIR_LOG2_FOLDING_FACTOR = 2;      // stark.rs:2023
 struct StirDerived {          // stir.rs:112-147
@@ -52,6 +56,23 @@ struct ClaimView {            // proof.rs:68-88, canonical words
   const u64 *input; size_t num_input;
   const u64 *output; size_t num_output;
 };
+inline ClaimView claim_view(const tvm_claim &c) { return {c.program_digest, c.version, c.input, c.num_input, c.output, c.num_output}; }
+// proof.rs:68-88: a claim's words are field elements; NULL with a non-zero count or a word >= p is an argument error (a
+// non-canonical word would otherwise alias the claim [x] with [x + p] in the transcript)
+inline bool claim_ok(const tvm_claim *c) {
+  if ((c->num_input && !c->input) || (c->num_output && !c->output)) return false;
+  for (int i = 0; i < 5; i++) if (c->program_digest[i] >= P) return false;
+  for (size_t i = 0; i < c->num_input; i++) if (c->input[i] >= P) return false;
+  for (size_t i = 0; i < c->num_output; i++) if (c->output[i] >= P) return false;
+  return true;
+}
+// `text` into the caller's failure buffer of `capacity` bytes, truncated and NUL-terminated (nothing without a buffer)
+inline void set_failure(char *failure, size_t capacity, const char *text) {
+  if (!failure || !capacity) return;
+  const size_t n = strnlen(text, capacity - 1);
+  memcpy(failure, text, n);
+  failure[n] = 0;
+}
 // Challenges::new (challenges.rs:88-135): appends the 4 challenges derived from the claim and the lookup table to the 59
 // sampled ones (Montgomery form), which gives the 63 in the order the AIR reads them
 void challenges_derive(const ClaimView &claim, std::vector<xfe> &ch);
@@ -65,22 +86,36 @@ struct ProveTimings {
   bool low_memory = false;                             // the last prove() ran in low-memory (just-in-time LDE) mode
 };
 
-// Table stages on the device (tvm_prove_tables): MasterMainTable::extend (master_table.rs:1006-1075) runs inside the prove
-// on the resident main trace instead of in a host callback; optionally the 230 degree-lowering main columns
-// (fill_derived_main_columns, substitutions.rs:128-161) are computed on the device too and never uploaded.
-struct DeviceTables {
-  const u64 *aux_rand;            // [91][h][3] canonical (host or device)
-  const u64 *randomizer_column;   // [n][3] canonical: aux column 90 (master_table.rs:1019-1025); nullptr = zeros
-  bool fill_derived_main;         // columns 149..378 of the main trace are computed, not read
-  const tvm_aet *aet = nullptr;   // the nine tables' columns come from the AET (main_fill.cu), no main trace is read at all
+// Where a prove's witness comes from.  Every array is canonical, in host or device memory.
+// Without an aux callback the table stages run on the device ("device-table mode", tvm_prove_tables): MasterMainTable::extend
+// (master_table.rs:1006-1075) runs inside the prove on the resident main trace; optionally the 230 degree-lowering main
+// columns (fill_derived_main_columns, substitutions.rs:128-161) are computed on the device too and never uploaded.
+struct ProveInputs {
+  const u64 *main_trace = nullptr;          // [379][n]; only columns 0..148 are read with fill_derived_main
+  const tvm_aet *aet = nullptr;             // device-table mode: the nine tables' columns come from the AET (main_fill.cu), no main trace is read
+  bool fill_derived_main = false;           // device-table mode: columns 149..378 of the main trace are computed, not read
+  AuxCallback aux_cb = nullptr;             // the caller extends the table; nullptr = device-table mode
+  void *aux_user = nullptr;
+  const u64 *main_rand = nullptr;           // [379][h]
+  const u64 *aux_rand = nullptr;            // device-table mode: [91][h][3] (the callback hands back its own)
+  const u64 *randomizer_column = nullptr;   // device-table mode: [n][3] aux column 90 (master_table.rs:1019-1025); nullptr = zeros
+  const u64 *quot_rand = nullptr;           // [nq][3]
+  const struct ExternalTranscript *ext = nullptr;   // the caller keeps the Fiat-Shamir transcript (tvm_prove_transcript)
 };
 
-void stark_prove(Ctx &c, const StarkParams &sp, const ClaimView &claim, size_t padded_height, const u64 *h_main_trace,
-                 const u64 *h_main_rand, AuxCallback aux_cb, void *aux_user, const u64 *h_quot_rand, std::vector<u64> &proof,
-                 ProveTimings *timings, const DeviceTables *dev_tables = nullptr, const struct ExternalTranscript *ext = nullptr);
+void stark_prove(Ctx &c, const StarkParams &sp, const ClaimView &claim, size_t padded_height, const ProveInputs &in,
+                 std::vector<u64> &proof, ProveTimings *timings);
 
 // ---- main_fill.cu: MasterMainTable::new + pad from the AET; d_table [>= 149][n] receives CANONICAL columns ----
 void main_fill_run(Ctx &c, struct DevMem &mem, const tvm_aet &aet, size_t n, u64 *d_table, uint64_t *lengths9);
+// the witness's main trace from the AET: d_main [379][n] Montgomery (the fill's scratch is released before it returns);
+// lengths9 (optional, host) receives the nine tables' lengths
+void main_table_on_device(Ctx &c, u64 *d_main, size_t n, const tvm_aet &aet, uint64_t *lengths9 = nullptr);
+// MasterMainTable::extend on the device: d_main [379][n] and d_ch [63*3] Montgomery (device) -> d_aux planes [273][n]
+// Montgomery.  The planes of column 90 receive randomizer_column ([n][3] canonical, host or device), or zeros without it.
+// The scratch comes from `mem` and goes back to it before this returns.
+void aux_extend_on_device(Ctx &c, struct DevMem &mem, const u64 *d_main, size_t n, const u64 *d_ch, const u64 *randomizer_column,
+                          u64 *d_aux);
 void bezout_run(Ctx &c, struct DevMem &mem, const u64 *d_roots_mont, size_t m, u64 *d_a, u64 *d_b);
 // the three hash traces of an execution (fill/hash_trace.cuh) into device memory of `mem`: d_out[section] [rows][67] canonical
 void hash_trace_run(Ctx &c, struct DevMem &mem, const tvm_execution &ex, u64 *d_out[3]);

@@ -721,14 +721,8 @@ extern "C" int tvm_stir_verify(uint32_t security_level, uint32_t soundness, uint
                                uint32_t log2_high_degree_bound, const uint64_t *proof, size_t proof_len, uint32_t *indices_out,
                                uint64_t *values_out, size_t *num_indices, char *failure, size_t failure_capacity) {
   using namespace tvm;
-  if (failure && failure_capacity) failure[0] = 0;
+  set_failure(failure, failure_capacity, "");
   if (!proof || !proof_len || soundness > 1) return TVM_ERR_INVALID_ARG;
-  auto report = [&](const char *what) {
-    if (failure && failure_capacity) {
-      std::strncpy(failure, what, failure_capacity - 1);
-      failure[failure_capacity - 1] = 0;
-    }
-  };
   StarkDerived d{};
   if (int rc = stir_derive(security_level, STIR_LOG2_FOLDING_FACTOR, log2_initial_expansion_factor, log2_high_degree_bound, soundness == 1,
                            d.stir))
@@ -751,13 +745,13 @@ extern "C" int tvm_stir_verify(uint32_t security_level, uint32_t soundness, uint
     }
     return TVM_OK;
   } catch (const VerifyFailure &f) {
-    report(f.what);
+    set_failure(failure, failure_capacity, f.what);
     return TVM_ERR_VERIFICATION;
   } catch (const std::exception &e) {
-    report(e.what());
+    set_failure(failure, failure_capacity, e.what());
     return TVM_ERR_VERIFICATION;
   } catch (...) {
-    report("internal error");
+    set_failure(failure, failure_capacity, "internal error");
     return TVM_ERR_VERIFICATION;
   }
 }
@@ -767,22 +761,16 @@ extern "C" int tvm_fri_verify(uint32_t security_level, uint32_t soundness, uint3
                               uint32_t log2_high_degree_bound, const uint64_t *proof, size_t proof_len, uint32_t *indices_out,
                               uint64_t *values_out, size_t *num_indices, char *failure, size_t failure_capacity) {
   using namespace tvm;
-  if (failure && failure_capacity) failure[0] = 0;
+  set_failure(failure, failure_capacity, "");
   if (!proof || !proof_len || soundness > 1) return TVM_ERR_INVALID_ARG;
-  auto report = [&](const char *what) {
-    if (failure && failure_capacity) {
-      std::strncpy(failure, what, failure_capacity - 1);
-      failure[failure_capacity - 1] = 0;
-    }
-  };
   FriDerived d{};
   const char *why = "";
   if (int rc = fri_derive(security_level, soundness == 1, log2_initial_expansion_factor, log2_high_degree_bound, d, &why)) {
-    report(why);
+    set_failure(failure, failure_capacity, why);
     return rc;
   }
   if (d.domain_len > ((size_t)1 << 31)) {   // ProofStream::sample_indices takes upper bounds up to u32::MAX (proof_stream.rs:85-89)
-    report("ProofStream::sample_indices: upper bound exceeds u32::MAX");
+    set_failure(failure, failure_capacity, "ProofStream::sample_indices: upper bound exceeds u32::MAX");
     return TVM_ERR_DOMAIN;
   }
   try {
@@ -800,13 +788,13 @@ extern "C" int tvm_fri_verify(uint32_t security_level, uint32_t soundness, uint3
     }
     return TVM_OK;
   } catch (const VerifyFailure &f) {
-    report(f.what);
+    set_failure(failure, failure_capacity, f.what);
     return TVM_ERR_VERIFICATION;
   } catch (const std::exception &e) {
-    report(e.what());
+    set_failure(failure, failure_capacity, e.what());
     return TVM_ERR_VERIFICATION;
   } catch (...) {
-    report("internal error");
+    set_failure(failure, failure_capacity, "internal error");
     return TVM_ERR_VERIFICATION;
   }
 }
@@ -833,31 +821,19 @@ extern "C" int tvm_proof_padded_height(const uint64_t *proof, size_t proof_len, 
 extern "C" int tvm_verify(const tvm_params *params, const tvm_claim *claim, const uint64_t *proof, size_t proof_len, int skip_air_check,
                           char *failure, size_t failure_capacity) {
   using namespace tvm;
-  if (failure && failure_capacity) failure[0] = 0;
-  if (!params || !claim || !proof || !proof_len || params->ldt_choice > 2) return TVM_ERR_INVALID_ARG;
-  if ((claim->num_input && !claim->input) || (claim->num_output && !claim->output)) return TVM_ERR_INVALID_ARG;
-  for (int i = 0; i < 5; i++) if (claim->program_digest[i] >= P) return TVM_ERR_INVALID_ARG;
-  for (size_t i = 0; i < claim->num_input; i++) if (claim->input[i] >= P) return TVM_ERR_INVALID_ARG;
-  for (size_t i = 0; i < claim->num_output; i++) if (claim->output[i] >= P) return TVM_ERR_INVALID_ARG;
-  auto report = [&](const char *what) {
-    if (failure && failure_capacity) {
-      std::strncpy(failure, what, failure_capacity - 1);
-      failure[failure_capacity - 1] = 0;
-    }
-  };
+  set_failure(failure, failure_capacity, "");
+  if (!params || !claim || !proof || !proof_len || params->ldt_choice > 2 || !claim_ok(claim)) return TVM_ERR_INVALID_ARG;
   try {
-    ClaimView cv{claim->program_digest, claim->version, claim->input, claim->num_input, claim->output, claim->num_output};
-    stark_verify(StarkParams{params->security_level, params->log2_ldt_expansion_factor, params->ldt_choice, params->soundness}, cv, proof,
-                 proof_len, !skip_air_check);
+    stark_verify(stark_params(*params), claim_view(*claim), proof, proof_len, !skip_air_check);
     return TVM_OK;
   } catch (const VerifyFailure &f) {
-    report(f.what);
+    set_failure(failure, failure_capacity, f.what);
     return TVM_ERR_VERIFICATION;
   } catch (const std::exception &e) {
-    report(e.what());
+    set_failure(failure, failure_capacity, e.what());
     return TVM_ERR_VERIFICATION;
   } catch (...) {
-    report("internal error");
+    set_failure(failure, failure_capacity, "internal error");
     return TVM_ERR_VERIFICATION;
   }
 }

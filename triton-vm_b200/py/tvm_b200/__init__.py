@@ -249,50 +249,40 @@ def lib():
     return _lib
 
 
-def stir_verify(security_level, log2_expansion, log2_high_degree_bound, proof, conjectured=False):
-    """Stir::verify for arbitrary StirParameters (host code, no GPU) -> (accepted, failure, first-round indices, partial first codeword [k,3])"""
+def _ldt_verify(entry, cap, security_level, log2_expansion, log2_high_degree_bound, proof, conjectured):
+    """a stand-alone low-degree test's verifier (tvm_stir_verify / tvm_fri_verify) with room for `cap` revealed indices"""
     pr, prp = _np_u64(proof)
-    cap = ctypes.c_size_t(8192)
-    idx = (ctypes.c_uint32 * 8192)()
-    vals = np.zeros((8192, 3), dtype=np.uint64)
+    icap = ctypes.c_size_t(cap)
+    idx = (ctypes.c_uint32 * cap)()
+    vals = np.zeros((cap, 3), dtype=np.uint64)
     msg = ctypes.create_string_buffer(256)
-    rc = lib().tvm_stir_verify(security_level, int(conjectured), log2_expansion, log2_high_degree_bound, prp, pr.size, idx,
-                               vals.ctypes.data_as(_u64p), ctypes.byref(cap), msg, 256)
+    rc = entry(security_level, int(conjectured), log2_expansion, log2_high_degree_bound, prp, pr.size, idx, vals.ctypes.data_as(_u64p),
+               ctypes.byref(icap), msg, 256)
     if rc == 0:
-        k = cap.value
+        k = icap.value
         return True, "", [int(idx[i]) for i in range(k)], vals[:k].copy()
     if rc == -9:
         return False, msg.value.decode(), [], vals[:0]
-    raise TvmError(rc, lib().tvm_strerror(rc).decode())
+    _check_plain(rc, msg.value.decode())
+
+
+def stir_verify(security_level, log2_expansion, log2_high_degree_bound, proof, conjectured=False):
+    """Stir::verify for arbitrary StirParameters (host code, no GPU) -> (accepted, failure, first-round indices, partial first codeword [k,3])"""
+    return _ldt_verify(lib().tvm_stir_verify, 8192, security_level, log2_expansion, log2_high_degree_bound, proof, conjectured)
 
 
 def fri_derive(security_level, log2_expansion, log2_high_degree_bound, conjectured=False):
     """FriParameters::try_into_fri + Fri::{max_degree, num_rounds, last_round_max_degree} (host code, no GPU) -> dict of
     tvm_fri_info's fields; raises TvmError (TVM_ERR_LDT_PARAMS = -6) for parameters the reference rejects"""
     out = FriInfo()
-    rc = lib().tvm_fri_derive(security_level, int(conjectured), log2_expansion, log2_high_degree_bound, ctypes.byref(out))
-    if rc:
-        raise TvmError(rc, lib().tvm_strerror(rc).decode())
+    _check_plain(lib().tvm_fri_derive(security_level, int(conjectured), log2_expansion, log2_high_degree_bound, ctypes.byref(out)))
     return {n: int(getattr(out, n)) for n, _ in FriInfo._fields_}
 
 
 def fri_verify(security_level, log2_expansion, log2_high_degree_bound, proof, conjectured=False):
     """Fri::verify for arbitrary FriParameters (host code, no GPU) -> (accepted, failure, first-round indices, partial first
     codeword [k,3]).  Parameter errors raise TvmError."""
-    pr, prp = _np_u64(proof)
-    cap = 1 << 16
-    icap = ctypes.c_size_t(cap)
-    idx = (ctypes.c_uint32 * cap)()
-    vals = np.zeros((cap, 3), dtype=np.uint64)
-    msg = ctypes.create_string_buffer(256)
-    rc = lib().tvm_fri_verify(security_level, int(conjectured), log2_expansion, log2_high_degree_bound, prp, pr.size, idx,
-                              vals.ctypes.data_as(_u64p), ctypes.byref(icap), msg, 256)
-    if rc == 0:
-        k = icap.value
-        return True, "", [int(idx[i]) for i in range(k)], vals[:k].copy()
-    if rc == -9:
-        return False, msg.value.decode(), [], vals[:0]
-    raise TvmError(rc, lib().tvm_strerror(rc).decode() + " | " + msg.value.decode())
+    return _ldt_verify(lib().tvm_fri_verify, 1 << 16, security_level, log2_expansion, log2_high_degree_bound, proof, conjectured)
 
 
 def _proof_capacity(dom):
@@ -305,6 +295,39 @@ def _proof_capacity(dom):
         est += sum(q * (16 + 5 * height) + 64 for q, _ in dom["stir_round_queries"]) + \
             dom["stir_final_num_queries"] * (16 + 5 * height) + 3 * (dom["stir_final_degree"] + 2) + 1024
     return est
+
+
+def _params(security_level, log2_expansion, ldt_choice, conjectured):
+    return Params(security_level, log2_expansion, ldt_choice, int(conjectured))
+
+
+def _claim(claim):
+    """claim = (program_digest[5], input, output[, version]) -> (ClaimStruct, the arrays it points into: keep them alive)"""
+    digest, inp, out = claim[0], claim[1], claim[2]
+    version = claim[3] if len(claim) > 3 else 6
+    ia, iap = _np_u64(np.array(list(inp), dtype=np.uint64))
+    oa, oap = _np_u64(np.array(list(out), dtype=np.uint64))
+    return ClaimStruct((ctypes.c_uint64 * 5)(*[int(v) for v in digest]), version, iap, ia.size, oap, oa.size), (ia, oa)
+
+
+def _aux_trampoline(aux_provider, n, h, keep, err):
+    """the AUX_CALLBACK of tvm_prove / tvm_prove_transcript: aux_provider(challenges [63,3]) -> (aux_trace [91, n, 3],
+    aux_rand [91, h, 3]) handed to the library zero-copy; `keep` holds them alive, `err` receives what aux_provider raised
+    (an exception must not propagate through the C frame)"""
+    def cb(_user, ch_p, trace_pp, rand_pp):
+        try:
+            t, r = aux_provider(np.ctypeslib.as_array(ch_p, shape=(63, 3)).copy())
+            t, tp, ts = _u64_arg(t)
+            r, rp, rs = _u64_arg(r)
+            assert int(np.prod(ts)) == 91 * n * 3 and int(np.prod(rs)) == 91 * h * 3, (ts, rs)
+            keep.extend([t, r])           # redirect to the caller's buffers (zero copy)
+            trace_pp[0] = tp
+            rand_pp[0] = rp
+            return 0
+        except Exception as e:  # noqa: BLE001 - must not propagate through the C frame
+            err.append(e)
+            return 1
+    return AUX_CALLBACK(cb)
 
 
 def _u64_arg(x):
@@ -325,9 +348,7 @@ def hash_varlen(words):
     """Tip5::hash_varlen on the host (no GPU needed)."""
     w, wp = _np_u64(np.array(words, dtype=np.uint64))
     d = np.zeros(5, dtype=np.uint64)
-    rc = lib().tvm_tip5_hash_varlen(wp, w.size, d.ctypes.data_as(_u64p))
-    if rc:
-        raise TvmError(rc, lib().tvm_strerror(rc).decode())
+    _check_plain(lib().tvm_tip5_hash_varlen(wp, w.size, d.ctypes.data_as(_u64p)))
     return [int(v) for v in d]
 
 
@@ -449,28 +470,22 @@ def _air_check_result(counts, first, last, arrays):
 
 def derive_domains(security_level=160, log2_expansion=2, padded_height=1 << 10, ldt_choice=LDT_AUTO, conjectured=False):
     """Stark::{fri, stir, max_degree, ...} + ProverDomains::derive; pure host function."""
-    p = Params(security_level, log2_expansion, ldt_choice, int(conjectured))
     d = Domains()
-    rc = lib().tvm_derive_domains(ctypes.byref(p), padded_height, ctypes.byref(d))
-    if rc:
-        raise TvmError(rc, lib().tvm_strerror(rc).decode())
+    _check_plain(lib().tvm_derive_domains(ctypes.byref(_params(security_level, log2_expansion, ldt_choice, conjectured)), padded_height,
+                                          ctypes.byref(d)))
     return d.as_dict()
 
 
 def verify(claim, proof, security_level=160, log2_expansion=2, ldt_choice=LDT_AUTO, conjectured=False, skip_air_check=False):
     """Stark::verify (tvm_verify; host code, no GPU needed).  claim = (program_digest[5], input, output[, version]);
     proof: the proof words.  Returns (accepted: bool, failure: str) — failure names the reference's error variant."""
-    digest, inp, out = claim[0], claim[1], claim[2]
-    version = claim[3] if len(claim) > 3 else 6
-    ia, iap = _np_u64(np.array(list(inp), dtype=np.uint64))
-    oa, oap = _np_u64(np.array(list(out), dtype=np.uint64))
-    cs = ClaimStruct((ctypes.c_uint64 * 5)(*[int(v) for v in digest]), version, iap, ia.size, oap, oa.size)
-    p = Params(security_level, log2_expansion, ldt_choice, int(conjectured))
+    cs, keep = _claim(claim)
+    p = _params(security_level, log2_expansion, ldt_choice, conjectured)
     pw, pwp = _np_u64(np.array(proof, dtype=np.uint64))
     buf = ctypes.create_string_buffer(256)
     rc = lib().tvm_verify(ctypes.byref(p), ctypes.byref(cs), pwp, pw.size, int(skip_air_check), buf, 256)
-    if rc not in (0, -9):
-        raise TvmError(rc, lib().tvm_strerror(rc).decode())
+    if rc != -9:
+        _check_plain(rc)
     return rc == 0, buf.value.decode()
 
 
@@ -480,19 +495,16 @@ def verify_batch(claims, proofs, security_level=160, log2_expansion=2, ldt_choic
     assert len(claims) == len(proofs)
     keep, cs = [], (ClaimStruct * len(claims))()
     for i, claim in enumerate(claims):
-        digest, inp, out = claim[0], claim[1], claim[2]
-        ia, iap = _np_u64(np.array(list(inp), dtype=np.uint64))
-        oa, oap = _np_u64(np.array(list(out), dtype=np.uint64))
-        keep += [ia, oa]
-        cs[i] = ClaimStruct((ctypes.c_uint64 * 5)(*[int(v) for v in digest]), claim[3] if len(claim) > 3 else 6, iap, ia.size, oap, oa.size)
+        cs[i], k = _claim(claim)
+        keep.append(k)
     arrs = [np.ascontiguousarray(np.array(p_, dtype=np.uint64)) for p_ in proofs]
     ptrs = (_u64p * len(arrs))(*[a.ctypes.data_as(_u64p) for a in arrs])
     lens = (ctypes.c_size_t * len(arrs))(*[a.size for a in arrs])
     res = (ctypes.c_int * len(arrs))()
-    p = Params(security_level, log2_expansion, ldt_choice, int(conjectured))
+    p = _params(security_level, log2_expansion, ldt_choice, conjectured)
     rc = lib().tvm_verify_batch(ctypes.byref(p), cs, ptrs, lens, len(arrs), int(skip_air_check), num_threads, res)
-    if rc not in (0, -9):
-        raise TvmError(rc, lib().tvm_strerror(rc).decode())
+    if rc != -9:
+        _check_plain(rc)
     return [r == 0 for r in res]
 
 
@@ -500,9 +512,7 @@ def proof_padded_height(proof):
     """Proof::padded_height; raises TvmError if the proof does not decode or holds no / several Log2PaddedHeight items"""
     pw, pwp = _np_u64(np.array(proof, dtype=np.uint64))
     out = ctypes.c_uint64(0)
-    rc = lib().tvm_proof_padded_height(pwp, pw.size, ctypes.byref(out))
-    if rc:
-        raise TvmError(rc, lib().tvm_strerror(rc).decode())
+    _check_plain(lib().tvm_proof_padded_height(pwp, pw.size, ctypes.byref(out)))
     return int(out.value)
 
 
@@ -512,9 +522,7 @@ class Backend:
     def __init__(self, device=0):
         self._l = lib()
         h = _vp()
-        rc = self._l.tvm_ctx_create(ctypes.byref(h), device)
-        if rc:
-            raise TvmError(rc, self._l.tvm_strerror(rc).decode())
+        _check_plain(self._l.tvm_ctx_create(ctypes.byref(h), device))
         self._h = h
         self.device = device
 
@@ -532,6 +540,22 @@ class Backend:
     def _chk(self, rc):
         if rc:
             raise TvmError(rc, self._l.tvm_strerror(rc).decode() + " | " + self._l.tvm_last_error(self._h).decode())
+
+    def _prove_into_buffer(self, call, dom):
+        """call(proof_out, proof_len) -> rc of a tvm_prove* entry point, into a buffer sized by _proof_capacity(dom).  When the
+        library reports a longer proof (rc == -1 and the required length in proof_len) the prove runs once more into a buffer
+        of that size.  -> the proof words"""
+        est = _proof_capacity(dom)
+        for _ in range(2):
+            buf = np.empty(est, dtype=np.uint64)
+            cap = ctypes.c_size_t(est)
+            rc = call(buf.ctypes.data_as(_u64p), ctypes.byref(cap))
+            if rc == -1 and cap.value > est:    # the proof is longer than the estimate: prove again into a buffer that fits
+                est = cap.value
+                continue
+            break
+        self._chk(rc)
+        return buf[:cap.value].copy()
 
     @property
     def launches(self):
@@ -631,41 +655,17 @@ class Backend:
         h = dom["num_trace_randomizers"]
         assert mt_shape == (379, dom["trace_len"]) and mr_shape == (379, h), (mt_shape, mr_shape, dom)
         assert qr.size == 3 * dom["num_quotient_randomizer_coefficients"]
-        digest, inp, out = claim[0], claim[1], claim[2]
-        version = claim[3] if len(claim) > 3 else 6
-        ia, iap = _np_u64(np.array(list(inp), dtype=np.uint64))
-        oa, oap = _np_u64(np.array(list(out), dtype=np.uint64))
-        cs = ClaimStruct((ctypes.c_uint64 * 5)(*[int(v) for v in digest]), version, iap, ia.size, oap, oa.size)
-        err = []
+        cs, keep_claim = _claim(claim)
+        p = _params(security_level, log2_expansion, ldt_choice, conjectured)
+        err, keep = [], []
+        cb = _aux_trampoline(aux_provider, n, h, keep, err)
 
-        keep = []
-
-        def cb(_user, ch_p, trace_pp, rand_pp):
-            try:
-                ch = np.ctypeslib.as_array(ch_p, shape=(63, 3)).copy()
-                t, r = aux_provider(ch)
-                t, tp, ts = _u64_arg(t)
-                r, rp, rs = _u64_arg(r)
-                assert int(np.prod(ts)) == 91 * n * 3 and int(np.prod(rs)) == 91 * h * 3, (ts, rs)
-                keep.extend([t, r])           # redirect to the caller's buffers (zero copy)
-                trace_pp[0] = tp
-                rand_pp[0] = rp
-                return 0
-            except Exception as e:  # noqa: BLE001 - must not propagate through the C frame
-                err.append(e)
-                return 1
-
-        p = Params(security_level, log2_expansion, ldt_choice, int(conjectured))
-        cap = ctypes.c_size_t(0)
-        est = _proof_capacity(dom)
-        buf = np.empty(est, dtype=np.uint64)
-        cap.value = est
-        rc = self._l.tvm_prove(self._h, ctypes.byref(p), ctypes.byref(cs), ph, mtp, mrp, AUX_CALLBACK(cb), None, qrp,
-                               buf.ctypes.data_as(_u64p), ctypes.byref(cap))
-        if err:
-            raise err[0]
-        self._chk(rc)
-        return buf[:cap.value].copy()
+        def call(proof_out, proof_len):
+            rc = self._l.tvm_prove(self._h, ctypes.byref(p), ctypes.byref(cs), ph, mtp, mrp, cb, None, qrp, proof_out, proof_len)
+            if err:
+                raise err[0]
+            return rc
+        return self._prove_into_buffer(call, dom)
 
     def prove_transcript(self, claim, main_trace, main_rand, aux_provider, quot_rand, transcript, security_level=160, log2_expansion=2,
                          padded_height=None, ldt_choice=LDT_AUTO, conjectured=False):
@@ -679,26 +679,9 @@ class Backend:
         ph = padded_height or n
         dom = derive_domains(security_level, log2_expansion, ph, ldt_choice, conjectured)
         h = dom["num_trace_randomizers"]
-        digest, inp, out = claim[0], claim[1], claim[2]
-        version = claim[3] if len(claim) > 3 else 6
-        ia, iap = _np_u64(np.array(list(inp), dtype=np.uint64))
-        oa, oap = _np_u64(np.array(list(out), dtype=np.uint64))
-        cs = ClaimStruct((ctypes.c_uint64 * 5)(*[int(v) for v in digest]), version, iap, ia.size, oap, oa.size)
+        cs, keep_claim = _claim(claim)
         err, keep = [], []
-
-        def cb(_user, ch_p, trace_pp, rand_pp):
-            try:
-                t, r = aux_provider(np.ctypeslib.as_array(ch_p, shape=(63, 3)).copy())
-                t, tp, ts = _u64_arg(t)
-                r, rp, rs = _u64_arg(r)
-                assert int(np.prod(ts)) == 91 * n * 3 and int(np.prod(rs)) == 91 * h * 3, (ts, rs)
-                keep.extend([t, r])
-                trace_pp[0] = tp
-                rand_pp[0] = rp
-                return 0
-            except Exception as e:  # noqa: BLE001
-                err.append(e)
-                return 1
+        cb = _aux_trampoline(aux_provider, n, h, keep, err)
 
         def guard(fn):
             def wrapped(*a):
@@ -727,8 +710,8 @@ class Backend:
         class T(ctypes.Structure):
             _fields_ = [("user", ctypes.c_void_p), ("abs", F_ABS), ("enq", F_ENQ), ("sca", F_SCA), ("idx", F_IDX)]
         ts_ = T(None, F_ABS(guard(f_abs)), F_ENQ(guard(f_enq)), F_SCA(guard(f_sca)), F_IDX(guard(f_idx)))
-        p = Params(security_level, log2_expansion, ldt_choice, int(conjectured))
-        rc = self._l.tvm_prove_transcript(self._h, ctypes.byref(p), ctypes.byref(cs), ph, mtp, mrp, AUX_CALLBACK(cb), None, qrp,
+        p = _params(security_level, log2_expansion, ldt_choice, conjectured)
+        rc = self._l.tvm_prove_transcript(self._h, ctypes.byref(p), ctypes.byref(cs), ph, mtp, mrp, cb, None, qrp,
                                           ctypes.cast(ctypes.byref(ts_), ctypes.c_void_p))
         if err:
             raise err[0]
@@ -754,19 +737,11 @@ class Backend:
         if randomizer_column is not None:
             rc_, rcp, rc_shape = _u64_arg(randomizer_column)
             assert int(np.prod(rc_shape)) == 3 * n
-        digest, inp, out = claim[0], claim[1], claim[2]
-        version = claim[3] if len(claim) > 3 else 6
-        ia, iap = _np_u64(np.array(list(inp), dtype=np.uint64))
-        oa, oap = _np_u64(np.array(list(out), dtype=np.uint64))
-        cs = ClaimStruct((ctypes.c_uint64 * 5)(*[int(v) for v in digest]), version, iap, ia.size, oap, oa.size)
-        p = Params(security_level, log2_expansion, ldt_choice, int(conjectured))
-        est = _proof_capacity(dom)
-        buf = np.empty(est, dtype=np.uint64)
-        cap = ctypes.c_size_t(est)
-        rc = self._l.tvm_prove_tables(self._h, ctypes.byref(p), ctypes.byref(cs), ph, mtp, int(bool(fill_derived_main_columns)), mrp, arp,
-                                      rcp, qrp, buf.ctypes.data_as(_u64p), ctypes.byref(cap))
-        self._chk(rc)
-        return buf[:cap.value].copy()
+        cs, keep_claim = _claim(claim)
+        p = _params(security_level, log2_expansion, ldt_choice, conjectured)
+        return self._prove_into_buffer(lambda proof_out, proof_len: self._l.tvm_prove_tables(
+            self._h, ctypes.byref(p), ctypes.byref(cs), ph, mtp, int(bool(fill_derived_main_columns)), mrp, arp, rcp, qrp, proof_out,
+            proof_len), dom)
 
     def main_table_from_aet(self, aet, num_rows):
         """tvm_main_table_from_aet: MasterMainTable::new + pad + degree-lowering columns on the device.
@@ -803,20 +778,12 @@ class Backend:
         if randomizer_column is not None:
             rc_, rcp, rc_shape = _u64_arg(randomizer_column)
             assert int(np.prod(rc_shape)) == 3 * n
-        digest, inp, out = claim[0], claim[1], claim[2]
-        version = claim[3] if len(claim) > 3 else 6
-        ia, iap = _np_u64(np.array(list(inp), dtype=np.uint64))
-        oa, oap = _np_u64(np.array(list(out), dtype=np.uint64))
-        cs = ClaimStruct((ctypes.c_uint64 * 5)(*[int(v) for v in digest]), version, iap, ia.size, oap, oa.size)
-        p = Params(security_level, log2_expansion, ldt_choice, int(conjectured))
-        est = _proof_capacity(dom)
-        buf = np.empty(est, dtype=np.uint64)
-        cap = ctypes.c_size_t(est)
-        rc = self._l.tvm_prove_aet(self._h, ctypes.byref(p), ctypes.byref(cs), ph, ctypes.byref(s), mrp, arp, rcp, qrp,
-                                   buf.ctypes.data_as(_u64p), ctypes.byref(cap))
-        del keep
-        self._chk(rc)
-        return buf[:cap.value].copy()
+        cs, keep_claim = _claim(claim)
+        p = _params(security_level, log2_expansion, ldt_choice, conjectured)
+        return self._prove_into_buffer(lambda proof_out, proof_len: self._l.tvm_prove_aet(
+            self._h, ctypes.byref(p), ctypes.byref(cs), ph, ctypes.byref(s), mrp, arp, rcp, qrp, proof_out, proof_len), dom)
+
+    _claim = staticmethod(_claim)   # the tests drive the C ABI with it directly
 
     @staticmethod
     def _seed(seed):
@@ -826,14 +793,6 @@ class Backend:
         seed = bytes(seed)
         assert len(seed) == 32, "the prover's randomness seed is 32 bytes"
         return seed
-
-    @staticmethod
-    def _claim(claim):
-        digest, inp, out = claim[0], claim[1], claim[2]
-        version = claim[3] if len(claim) > 3 else 6
-        ia, iap = _np_u64(np.array(list(inp), dtype=np.uint64))
-        oa, oap = _np_u64(np.array(list(out), dtype=np.uint64))
-        return ClaimStruct((ctypes.c_uint64 * 5)(*[int(v) for v in digest]), version, iap, ia.size, oap, oa.size), (ia, oa)
 
     def prover_randomness(self, seed, padded_height, security_level=160, log2_expansion=2, ldt_choice=LDT_AUTO, conjectured=False,
                           out=None):
@@ -856,7 +815,7 @@ class Backend:
             if isinstance(o, np.ndarray):
                 assert o.flags.c_contiguous and o.dtype == np.uint64
             ptrs.append(op)
-        p = Params(security_level, log2_expansion, ldt_choice, int(conjectured))
+        p = _params(security_level, log2_expansion, ldt_choice, conjectured)
         self._chk(self._l.tvm_prover_randomness(self._h, ctypes.byref(p), padded_height, self._seed(seed), *ptrs))
         return out
 
@@ -867,33 +826,18 @@ class Backend:
         s, keep = aet_struct(aet)
         ph = int(padded_height)
         dom = derive_domains(security_level, log2_expansion, ph, ldt_choice, conjectured)
-        cs, keep_claim = self._claim(claim)
-        p = Params(security_level, log2_expansion, ldt_choice, int(conjectured))
-        est = _proof_capacity(dom)
-        buf = np.empty(est, dtype=np.uint64)
-        cap = ctypes.c_size_t(est)
-        rc = self._l.tvm_prove_aet_seeded(self._h, ctypes.byref(p), ctypes.byref(cs), ph, ctypes.byref(s), self._seed(seed),
-                                          buf.ctypes.data_as(_u64p), ctypes.byref(cap))
-        del keep, keep_claim
-        self._chk(rc)
-        return buf[:cap.value].copy()
+        cs, keep_claim = _claim(claim)
+        p = _params(security_level, log2_expansion, ldt_choice, conjectured)
+        return self._prove_into_buffer(lambda proof_out, proof_len: self._l.tvm_prove_aet_seeded(
+            self._h, ctypes.byref(p), ctypes.byref(cs), ph, ctypes.byref(s), self._seed(seed), proof_out, proof_len), dom)
 
     def prove_execution(self, ex, seed, security_level=160, log2_expansion=2, ldt_choice=LDT_AUTO, conjectured=False):
         """tvm_prove_execution: Stark::prove of an Execution's claim from its AET (hash traces expanded on the device) and the
         prover's 32-byte randomness seed -> proof words.  The seed must come from a CSPRNG the verifier cannot predict."""
         dom = derive_domains(security_level, log2_expansion, ex.padded_height, ldt_choice, conjectured)
-        p = Params(security_level, log2_expansion, ldt_choice, int(conjectured))
-        est = _proof_capacity(dom)
-        for _ in range(2):
-            buf = np.empty(est, dtype=np.uint64)
-            cap = ctypes.c_size_t(est)
-            rc = self._l.tvm_prove_execution(self._h, ctypes.byref(p), ex._h, self._seed(seed), buf.ctypes.data_as(_u64p), ctypes.byref(cap))
-            if rc == -1 and cap.value > est:    # the proof is longer than the estimate: prove again into a buffer that fits
-                est = cap.value
-                continue
-            break
-        self._chk(rc)
-        return buf[:cap.value].copy()
+        p = _params(security_level, log2_expansion, ldt_choice, conjectured)
+        return self._prove_into_buffer(lambda proof_out, proof_len: self._l.tvm_prove_execution(
+            self._h, ctypes.byref(p), ex._h, self._seed(seed), proof_out, proof_len), dom)
 
     def prove_program(self, words, public_input=(), secret_input=(), digests=(), ram=None, seed=None, **params):
         """triton_vm::prove_program (lib.rs:228-267): trace the program on the host, prove on this GPU -> (claim, proof)"""
@@ -924,7 +868,7 @@ class Backend:
         """tvm_air_check_aet: the witness tvm_prove_aet builds from `aet` (fill, padding to num_rows, degree-lowering columns,
         Challenges::new from `claim` on the 59 sampled challenges [59, 3], extension) checked on the device; result as air_check"""
         s, keep = aet_struct(aet)
-        cs, keep_claim = self._claim(claim)
+        cs, keep_claim = _claim(claim)
         sp_, spp = _np_u64(np.asarray(sampled, dtype=np.uint64).reshape(59, 3))
         out = [_U64x604() for _ in range(3)]
         nv = ctypes.c_uint64()
@@ -960,16 +904,11 @@ class Backend:
         ph = padded_height or mt_shape[1]
         dom = derive_domains(security_level, log2_expansion, ph, ldt_choice, conjectured)
         assert mt_shape == (379, dom["trace_len"]), mt_shape
-        cs, keep_claim = self._claim(claim)
-        p = Params(security_level, log2_expansion, ldt_choice, int(conjectured))
-        est = _proof_capacity(dom)
-        buf = np.empty(est, dtype=np.uint64)
-        cap = ctypes.c_size_t(est)
-        rc = self._l.tvm_prove_tables_seeded(self._h, ctypes.byref(p), ctypes.byref(cs), ph, mtp, int(bool(fill_derived_main_columns)),
-                                             self._seed(seed), buf.ctypes.data_as(_u64p), ctypes.byref(cap))
-        del keep_claim
-        self._chk(rc)
-        return buf[:cap.value].copy()
+        cs, keep_claim = _claim(claim)
+        p = _params(security_level, log2_expansion, ldt_choice, conjectured)
+        return self._prove_into_buffer(lambda proof_out, proof_len: self._l.tvm_prove_tables_seeded(
+            self._h, ctypes.byref(p), ctypes.byref(cs), ph, mtp, int(bool(fill_derived_main_columns)), self._seed(seed), proof_out,
+            proof_len), dom)
 
     def stir_prove(self, security_level, log2_expansion, log2_high_degree_bound, codeword, conjectured=False):
         """Stir::prove on the device for arbitrary StirParameters: codeword [2^(hdb+exp), 3] canonical -> (proof words, revealed indices)"""
