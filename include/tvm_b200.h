@@ -119,6 +119,11 @@ int tvm_merkle_build_dev(tvm_ctx *ctx, uint64_t *d_nodes, size_t nleaves);
 int tvm_merkle_build(tvm_ctx *ctx, const uint64_t *leaves /* [nleaves][5] */, size_t nleaves,
                      uint64_t *nodes_out /* [2*nleaves][5] or NULL */, uint64_t root[5]);
 
+/* Kernel-level check of the Tip5 permutation's arithmetic (raw words, no Montgomery conversion): d_in [n][5] =
+ * (x, lo, hi, top, rc) with lo, hi < 2^47, top < 2^21; d_out [n][4] = (fsqr(x), the Tip5 power map x^7, the lazy MDS finish and the
+ * canonical MDS finish of lo + 2^32 hi + 2^64 top + rc). */
+int tvm_tip5_arith_check_dev(tvm_ctx *ctx, const uint64_t *d_in, size_t n, uint64_t *d_out);
+
 /* ---- AIR quotient codeword: all_quotients_combined (master_table.rs:1264-1363) with the
  *      build-time generated constraint evaluators (constraint-builder/src/codegen.rs:59-269)
  *      and the four zerofier inverses (master_table.rs:1194-1252).

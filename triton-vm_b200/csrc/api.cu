@@ -412,6 +412,14 @@ int tvm_merkle_build_dev(tvm_ctx *ctx, uint64_t *d_nodes, size_t nleaves) {
   TVM_API_END
 }
 
+int tvm_tip5_arith_check_dev(tvm_ctx *ctx, const uint64_t *d_in, size_t n, uint64_t *d_out) {
+  if (!ctx || (n && (!d_in || !d_out))) return TVM_ERR_INVALID_ARG;
+  TVM_API_BEGIN(ctx)
+  if (!n) return TVM_OK;
+  tip5_arith_check_run(*c__, (const u64 *)d_in, n, (u64 *)d_out);
+  TVM_API_END
+}
+
 int tvm_merkle_build(tvm_ctx *ctx, const uint64_t *leaves, size_t nleaves, uint64_t *nodes_out, uint64_t root[5]) {
   if (!ctx || !leaves || !root || nleaves == 0 || (nleaves & (nleaves - 1))) return TVM_ERR_INVALID_ARG;
   TVM_API_BEGIN(ctx)

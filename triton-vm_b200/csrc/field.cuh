@@ -31,6 +31,7 @@ static constexpr u64 EPS = 0xFFFFFFFFULL;               // 2^64 mod p
 // are bound by the integer-ALU pipe rather than by the IMAD (fma) pipe,
 // and the compiler's compare/select sequences for the C versions cost 13 ALU instructions per
 // fmul, 9 per fadd/fsub; the chains below cost 8 / 7 / 5.
+// Contract for ANY x < 2^128: the result is < 2^64 and congruent to x * 2^-64 (hi - b with b < p, plus p on borrow).
 TVM_HD u64 montyred(u64 lo, u64 hi) {
 #ifdef __CUDA_ARCH__
   u32 x0 = (u32)lo, x1 = (u32)(lo >> 32), x2 = (u32)hi, x3 = (u32)(hi >> 32);
@@ -69,7 +70,12 @@ TVM_HD u64 fmul(u64 a, u64 b) {
   u64 lo = (u64)x, hi = (u64)(x >> 64);
   return montyred(lo, hi);
 }
+// Squaring as the general product: a three-product form (a0^2 + 2^33 a0 a1 + 2^64 a1^2) saves one IMAD.WIDE but pays
+// for doubling the cross term with shifts and a separate carry chain; in the Tip5 round it measured 20 SASS instructions
+// MORE per round body (704 against 684 on sm_90a) than nvcc's four accumulating IMAD.WIDE.
 TVM_HD u64 fsqr(u64 a) { return fmul(a, a); }
+// the canonical representative of any x < 2^64
+TVM_HD u64 fcanon(u64 x) { return x >= P ? x - P : x; }
 
 TVM_HD u64 fsub(u64 a, u64 b) {  // canonical a, b in [0, p] -> canonical
 #ifdef __CUDA_ARCH__

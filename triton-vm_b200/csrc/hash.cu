@@ -205,13 +205,15 @@ __device__ __forceinline__ unsigned lookup_word(unsigned w, const unsigned char 
 __device__ __forceinline__ u64 lookup_u64(u64 v, const unsigned char *lut) {
   return ((u64)lookup_word((unsigned)(v >> 32), lut) << 32) | lookup_word((unsigned)v, lut);
 }
+// x^7 (in Montgomery form: x^7 R^-6) of any representative < 2^64, by montyred's contract; the result is < 2^64
+__device__ __forceinline__ u64 pow7(u64 x) {
+  const u64 x2 = fsqr(x), x3 = fmul(x2, x), x4 = fsqr(x2);
+  return fmul(x3, x4);
+}
 __device__ __forceinline__ void quad_sbox(u64 (&s)[4], const unsigned char *lut) {
-  s[0] = lookup_u64(s[0], lut);   // slot 0: split-and-lookup
+  s[0] = lookup_u64(s[0], lut);   // slot 0: split-and-lookup (canonical input)
 #pragma unroll
-  for (int i = 1; i < 4; i++) {
-    u64 x = s[i], x2 = fmul(x, x), x3 = fmul(x2, x), x4 = fmul(x2, x2);
-    s[i] = fmul(x3, x4);
-  }
+  for (int i = 1; i < 4; i++) s[i] = pow7(s[i]);
 }
 __device__ __forceinline__ void quad_mds_rc(u64 (&s)[4], int l, int group_base, const u64 *rc_smem, int rnd) {
   constexpr unsigned short MDS[16] = TVM_MDS_COL;
@@ -376,7 +378,7 @@ __global__ void __launch_bounds__(HASHQ2_THREADS) tip5_hash_rows_quad2_kernel(Ha
 // IS the IMMA A-fragment layout (fragment row g / g+8 = first / second row of quad g, fragment k = 4l+t = element
 // l+4t of lane l), and choosing the B-fragment column order as o(j, n) = (n >> 1) + 4 (2j + (n & 1)) makes the
 // D fragment of N-block j land on the lane that owns the output element: c0/c1 = elements l+8j, l+8j+4 of the first row,
-// c2/c3 of the second.  No shuffles, 18 IMMA + 64 IMAD.WIDE (limb recombination) per lane and round instead of
+// c2/c3 of the second.  No shuffles, 18 IMMA + 16 IMAD.WIDE and 32 IMAD (limb recombination) per lane and round instead of
 // 256 IMAD.WIDE + 64 SHFL + 64 SEL.  The M_0 / M_1 fragments are 4 constant registers per lane.
 __device__ __forceinline__ void imma_16832_u8(int (&d)[4], unsigned a0, unsigned a1, unsigned a2, unsigned a3, unsigned b0,
                                               unsigned b1) {
@@ -416,40 +418,63 @@ __device__ __forceinline__ void byte_transpose4(unsigned w0, unsigned w1, unsign
   o[0] = __byte_perm(t01l, t23l, 0x5410); o[1] = __byte_perm(t01l, t23l, 0x7632);
   o[2] = __byte_perm(t01h, t23h, 0x5410); o[3] = __byte_perm(t01h, t23h, 0x7632);
 }
-// lo + 2^32 hi + rc  (lo < 2^46, hi < 2^54, rc canonical) reduced to canonical form.  Four homogeneous carry chains
-// (16 instructions; the compare/select code nvcc emits for the C formulation is ~45):
-//   V = lo + rc + (hi << 32) = w0 + 2^32 w1 + 2^64 w2 (w2 < 2^23);  2^64 = 2^32 - 1 (mod p):  s = (w0, w1) - w2 + 2^32 w2
-//   tracked as s + n 2^64 with n in {0, 1} (a borrow of the subtraction is always cancelled by the carry of the addition);
-//   result = s + n 2^64 - p if that is >= 0, else s:  u = s + (2^32 - 1) and the carry / n select.
-__device__ __forceinline__ u64 mds_finish(u64 lo, u64 hi, u64 rc) {
-  u64 r;
+// V = lo + 2^32 hi + 2^64 top + rc  (lo, hi < 2^47, top < 2^21, rc < 2^64) folded to s + n 2^64 with s < 2^64, n in {0, 1}.
+// Homogeneous carry chains (the compare/select code nvcc emits for the C formulation is ~45 instructions):
+//   V = w0 + 2^32 w1 + 2^64 w2 (w2 < 2^23);  2^64 = 2^32 - 1 (mod p):  s + n 2^64 = (w0, w1) - w2 + 2^32 w2
+//   (a borrow of the subtraction is always cancelled by the carry of the addition, so n is 0 or 1, and n = 1 means
+//   s < 2^32 w2 < 2^55).
+struct MdsFold { u64 s; unsigned n; };
+__device__ __forceinline__ MdsFold mds_fold(u64 lo, u64 hi, unsigned top, u64 rc) {
+  unsigned s0, s1, n;
   asm("{\n\t"
-      ".reg .u32 l0, l1, h0, h1, r0, r1, w0, w1, w2, s0, s1, m, n, u0, u1, k;\n\t"
-      ".reg .pred q;\n\t"
-      "mov.b64 {l0, l1}, %1;\n\t"
-      "mov.b64 {h0, h1}, %2;\n\t"
-      "mov.b64 {r0, r1}, %3;\n\t"
+      ".reg .u32 l0, l1, h0, h1, r0, r1, w0, w1, w2, m;\n\t"
+      "mov.b64 {l0, l1}, %3;\n\t"
+      "mov.b64 {h0, h1}, %4;\n\t"
+      "mov.b64 {r0, r1}, %6;\n\t"
       "add.cc.u32 w0, l0, r0;\n\t"
       "addc.cc.u32 w1, l1, r1;\n\t"
-      "addc.u32 w2, h1, 0;\n\t"
+      "addc.u32 w2, h1, %5;\n\t"
       "add.cc.u32 w1, w1, h0;\n\t"
       "addc.u32 w2, w2, 0;\n\t"
-      "sub.cc.u32 s0, w0, w2;\n\t"
-      "subc.cc.u32 s1, w1, 0;\n\t"
+      "sub.cc.u32 %0, w0, w2;\n\t"
+      "subc.cc.u32 %1, w1, 0;\n\t"
       "subc.u32 m, 0, 0;\n\t"
-      "add.cc.u32 s1, s1, w2;\n\t"
-      "addc.u32 n, m, 0;\n\t"
+      "add.cc.u32 %1, %1, w2;\n\t"
+      "addc.u32 %2, m, 0;\n\t"
+      "}"
+      : "=r"(s0), "=r"(s1), "=r"(n)
+      : "l"(lo), "l"(hi), "r"(top), "l"(rc));
+  return {((u64)s1 << 32) | s0, n};
+}
+// canonical: s + n 2^64 - p if that is >= 0, else s  (u = s + (2^32 - 1), and the carry / n select).  For the look-up
+// element and for whatever leaves the permutation.
+__device__ __forceinline__ u64 mds_finish(u64 lo, u64 hi, unsigned top, u64 rc) {
+  const MdsFold f = mds_fold(lo, hi, top, rc);
+  u64 r;
+  asm("{\n\t"
+      ".reg .u32 s0, s1, u0, u1, k;\n\t"
+      ".reg .pred q;\n\t"
+      "mov.b64 {s0, s1}, %1;\n\t"
       "add.cc.u32 u0, s0, 0xffffffff;\n\t"
       "addc.cc.u32 u1, s1, 0;\n\t"
-      "addc.u32 k, n, 0;\n\t"
+      "addc.u32 k, %2, 0;\n\t"
       "setp.ne.u32 q, k, 0;\n\t"
       "selp.u32 s0, u0, s0, q;\n\t"
       "selp.u32 s1, u1, s1, q;\n\t"
       "mov.b64 %0, {s0, s1};\n\t"
       "}"
       : "=l"(r)
-      : "l"(lo), "l"(hi), "l"(rc));
+      : "l"(f.s), "r"(f.n));
   return r;
+}
+// lazy: a representative < 2^64, s + n (2^32 - 1) (no wrap: n = 1 implies s < 2^55), for the elements that only feed
+// the x^7 power map.  One IMAD.WIDE; the multiplier comes from constant memory so that ptxas keeps it one instruction.
+__constant__ unsigned c_eps32 = 0xFFFFFFFFu;
+__device__ __forceinline__ u64 mds_finish_lazy(u64 lo, u64 hi, unsigned top, u64 rc) {
+  const MdsFold f = mds_fold(lo, hi, top, rc);
+  u64 d;
+  asm("mad.wide.u32 %0, %1, %2, %3;" : "=l"(d) : "r"(f.n), "r"(c_eps32), "l"(f.s));
+  return d;
 }
 __device__ __forceinline__ void quad2_mds_mma(u64 (&a)[4], u64 (&b)[4], int l, const MdsFrag &f, const u64 *rc_smem, int rnd) {
   unsigned La[8], Lb[8];
@@ -468,11 +493,14 @@ __device__ __forceinline__ void quad2_mds_mma(u64 (&a)[4], u64 (&b)[4], int l, c
 #pragma unroll
     for (int i = 0; i < 4; i++) Lb[4 + i] = o[i];
   }
-  // 2^8, 2^16, 2^24 from constant memory, which neither nvcc nor ptxas folds: a literal power of two is strength-reduced
-  // from one IMAD.WIDE into SHL + HI + two carry adds
-  const unsigned pw[4] = {1u, c_pow256[1], c_pow256[2], c_pow256[3]};
-  // accumulators: [row a/b][t = 2j + c]
+  // Recombination y = sum_s 2^(8s) T_s (T_s < 2^21): pairs e = T_s + 2^8 T_{s+1} < 2^30 in 32 bits, then
+  // lo = e_01 + 2^16 e_23 and hi = e_45 + 2^16 e_67 (< 2^47) with one IMAD.WIDE each; T_8 goes to mds_fold as the
+  // 2^64 word.  2^8 and 2^16 come from constant memory, which neither nvcc nor ptxas folds: a literal power of two is
+  // strength-reduced from one IMAD into ALU shifts and carry adds.
+  const unsigned pw8 = c_pow256[1], pw16 = c_pow256[2];
+  // [row a/b][t = 2j + c]
   u64 lo[2][4], hi[2][4];
+  unsigned e0[2][4], e1[2][4], top[2][4];
 #pragma unroll
   for (int s = 0; s <= 8; s++) {
     const unsigned a0 = s < 8 ? La[s] : 0u, a1 = s < 8 ? Lb[s] : 0u;
@@ -485,21 +513,33 @@ __device__ __forceinline__ void quad2_mds_mma(u64 (&a)[4], u64 (&b)[4], int l, c
       for (int c = 0; c < 4; c++) {
         const int row = c >> 1, t = 2 * j + (c & 1);
         const unsigned v = (unsigned)d[c];
-        if (s == 0) lo[row][t] = v;
-        else if (s < 4) lo[row][t] = mad_wide(v, pw[s], lo[row][t]);
-        else if (s == 4) hi[row][t] = v;
-        else if (s < 8) hi[row][t] = mad_wide(v, pw[s - 4], hi[row][t]);
-        else hi[row][t] += (u64)v << 32;
+        if (s == 8) top[row][t] = v;
+        else if ((s & 3) == 0) e0[row][t] = v;
+        else if ((s & 3) == 1) e0[row][t] += v * pw8;
+        else if ((s & 3) == 2) e1[row][t] = v;
+        else {
+          const u64 w = mad_wide(e1[row][t] + v * pw8, pw16, (u64)e0[row][t]);
+          if (s == 3) lo[row][t] = w;
+          else hi[row][t] = w;
+        }
       }
     }
   }
+  // slot 0 feeds the next round's look-up and must be canonical; the x^7 slots take any representative < 2^64
 #pragma unroll
   for (int t = 0; t < 4; t++) {
     const u64 rc = rc_smem[16 * rnd + l + 4 * t];
-    a[t] = mds_finish(lo[0][t], hi[0][t], rc);
-    b[t] = mds_finish(lo[1][t], hi[1][t], rc);
+    if (t == 0) {
+      a[t] = mds_finish(lo[0][t], hi[0][t], top[0][t], rc);
+      b[t] = mds_finish(lo[1][t], hi[1][t], top[1][t], rc);
+    } else {
+      a[t] = mds_finish_lazy(lo[0][t], hi[0][t], top[0][t], rc);
+      b[t] = mds_finish_lazy(lo[1][t], hi[1][t], top[1][t], rc);
+    }
   }
 }
+// The state leaves in lazy form: slot 0 (elements 0..3) is canonical, slots 1..3 are representatives < 2^64.  Callers
+// canonicalise what they store (fcanon); capacity elements stay lazy from one absorption to the next.
 __device__ __forceinline__ void tip5_perm_quad2_mma(u64 (&a)[4], u64 (&b)[4], int l, const MdsFrag &f, const unsigned char *lut,
                                                     const u64 *rc_smem) {
 #pragma unroll 1
@@ -508,6 +548,25 @@ __device__ __forceinline__ void tip5_perm_quad2_mma(u64 (&a)[4], u64 (&b)[4], in
     quad_sbox(b, lut);
     quad2_mds_mma(a, b, l, f, rc_smem, rnd);
   }
+}
+
+// Kernel-level check of the permutation's arithmetic pieces: in [n][5] = (x, lo, hi, top, rc), out [n][4] =
+// (fsqr(x), pow7(x), mds_finish_lazy(lo, hi, top, rc), mds_finish(lo, hi, top, rc)).  Inputs outside the finish's
+// bounds (lo, hi < 2^47, top < 2^21) are the caller's error.
+__global__ void tip5_arith_check_kernel(const u64 *in, size_t n, u64 *out) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const u64 *v = in + 5 * i;
+  u64 *o = out + 4 * i;
+  o[0] = fsqr(v[0]);
+  o[1] = pow7(v[0]);
+  o[2] = mds_finish_lazy(v[1], v[2], (unsigned)v[3], v[4]);
+  o[3] = mds_finish(v[1], v[2], (unsigned)v[3], v[4]);
+}
+void tip5_arith_check_run(Ctx &c, const u64 *in, size_t n, u64 *out) {
+  tip5_arith_check_kernel<<<(unsigned)((n + 127) / 128), 128, 0, c.stream>>>(in, n, out);
+  c.launches++;
+  TVM_CUDA(cudaGetLastError());
 }
 
 static constexpr int HASHM_THREADS = 128;   // 32 quads, 64 rows per CTA
@@ -566,7 +625,7 @@ __global__ void __launch_bounds__(HASHM_THREADS) tip5_hash_rows_mma_kernel(HashR
     u64 *d = p.digests + (coset + (k << p.log_r)) * 5;
     const u64 *s = t ? b : a;
     d[l] = s[0];
-    if (l == 0) d[4] = s[1];
+    if (l == 0) d[4] = fcanon(s[1]);
   }
 }
 
@@ -671,7 +730,7 @@ __global__ void __launch_bounds__(HASHM_THREADS) tip5_hash_rows_mma_tma_kernel(H
     u64 *d = p.digests + (coset + (k << p.log_r)) * 5;
     const u64 *s = t ? b : a;
     d[l] = s[0];
-    if (l == 0) d[4] = s[1];
+    if (l == 0) d[4] = fcanon(s[1]);
   }
 }
 
@@ -706,7 +765,7 @@ __global__ void __launch_bounds__(HASHM_THREADS) merkle_level_mma_kernel(u64 *no
     if (!active[t]) continue;
     u64 *d = nodes + 5 * node[t];
     d[l] = s[t][0];
-    if (l == 0) d[4] = s[t][1];
+    if (l == 0) d[4] = fcanon(s[t][1]);
   }
 }
 

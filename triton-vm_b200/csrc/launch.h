@@ -49,6 +49,7 @@ bool lde_interpolate_tiles(Ctx &c, const u64 *d_trace, const u64 *d_rand, unsign
 void hash_rows_run(Ctx &c, const u64 *table, size_t col_stride, size_t nrows, unsigned ncols, int log_r, u64 *digests,
                    unsigned coset_mem_stride = 1);
 void merkle_run(Ctx &c, u64 *nodes, size_t nleaves);
+void tip5_arith_check_run(Ctx &c, const u64 *in, size_t n, u64 *out);   // fsqr and the MDS finishes, for tests
 void merkle_run_sharded(Ctx &c, u64 *nodes, size_t nleaves, unsigned rank, unsigned world);
 void xfe_leaves_run(Ctx &c, const u64 *cw, size_t stride, size_t n, u64 *leaves);
 void to_mont_run(Ctx &c, u64 *d, size_t n);

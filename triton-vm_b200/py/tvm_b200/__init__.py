@@ -185,6 +185,7 @@ _SIGNATURES = {
     "tvm_tip5_hash_varlen": (ctypes.c_int, [_u64p, ctypes.c_size_t, _u64p]),
     "tvm_merkle_build_dev": (ctypes.c_int, [_vp, _vp, ctypes.c_size_t]),
     "tvm_merkle_build": (ctypes.c_int, [_vp, _u64p, ctypes.c_size_t, _u64p, _u64p]),
+    "tvm_tip5_arith_check_dev": (ctypes.c_int, [_vp, _vp, ctypes.c_size_t, _vp]),
     "tvm_derive_domains": (ctypes.c_int, [ctypes.POINTER(Params), ctypes.c_uint64, ctypes.POINTER(Domains)]),
     "tvm_prove": (ctypes.c_int, [_vp, ctypes.POINTER(Params), ctypes.POINTER(ClaimStruct), ctypes.c_uint64, _u64p, _u64p,
                                  AUX_CALLBACK, _vp, _u64p, _u64p, ctypes.POINTER(ctypes.c_size_t)]),
@@ -1004,3 +1005,6 @@ class Backend:
 
     def merkle_dev(self, d_nodes, nleaves):
         self._chk(self._l.tvm_merkle_build_dev(self._h, self._dp(d_nodes), nleaves))
+
+    def tip5_arith_check_dev(self, d_in, n, d_out):
+        self._chk(self._l.tvm_tip5_arith_check_dev(self._h, self._dp(d_in), n, self._dp(d_out)))
