@@ -141,6 +141,13 @@ int tvm_air_quotient_dev(tvm_ctx *ctx, const uint64_t *d_main, size_t main_strid
                          size_t aux_stride, const uint64_t *challenges, const uint64_t *weights,
                          unsigned log2_trace, unsigned log2_cosets, uint64_t offset_canon,
                          uint64_t *d_out, size_t out_stride);
+/* The prover's quotient path from column polynomials, for tests at any (n, h): d_main_coef [379][coef_stride] and
+ * d_aux_coef [270][coef_stride] hold the coefficients (Montgomery, in x) of polynomials of degree < n + num_rand,
+ * num_rand <= n.  They are evaluated on the 8n-point quotient domain offset*<w_{8n}> and the quotient is computed as
+ * the prover does, with the degree split whenever the degrees allow it.  d_out as for tvm_air_quotient_dev (r = 8). */
+int tvm_air_quotient_coef_dev(tvm_ctx *ctx, const uint64_t *d_main_coef, const uint64_t *d_aux_coef, size_t coef_stride,
+                              unsigned num_rand, const uint64_t *challenges, const uint64_t *weights, unsigned log2_trace,
+                              uint64_t offset_canon, uint64_t *d_out, size_t out_stride);
 
 /* ---- STARK parameters: Stark::{ldt,fri,max_degree,randomized_trace_len,num_trace_randomizers}
  *      (stark.rs:1885-2089), ProverDomains::derive (263-286), FriParameters (fri.rs:799-924),

@@ -13,7 +13,8 @@ design (14 chunks of ~30k SASS instructions each) showed a low issue rate
 with `stalled_no_instruction` dominating - straight-line code that large streams through the
 32 KB L1.5 instruction cache once per warp.  A chunk is therefore sized to stay instruction-cache
 resident (budget below, ~25 SASS instructions per cost unit); a node needed by two chunks is
-recomputed and a chunk re-reads the table columns it touches, which HBM has ample headroom for.
+recomputed and a chunk re-reads the table columns it touches (on H100 that re-reading is a large part of the stage's HBM
+traffic: the degree split below halves it by evaluating every chunk on half of the rows).
 Every chunk adds its zerofier-weighted partial sum into the row-planar X-field output.  The
 weighted sum  sum_j w_j * c_j  is accumulated UNREDUCED (three 128-bit accumulators + overflow
 words, one Montgomery reduction per chunk instead of one per product); the per-weight linear map
@@ -40,13 +41,15 @@ MIN_BLOCKS = int(os.environ.get("TVM_AIR_MIN_BLOCKS", "2"))   # __launch_bounds_
 SPLIT_BIG = os.environ.get("TVM_AIR_SPLIT", "1") != "0"
 SPLIT_BUDGET = float(os.environ.get("TVM_AIR_SPLIT_BUDGET", "400"))   # pieces of an oversized constraint may be this large
 WTAB_WORDS = 7   # per weight: b0, b1, b2, -b1, -b2, b0+b2, b1-b2
-# Degree split: the trace polynomials have degree < 2n, so the weighted sum of the constraints of degree <= 2 of one zerofier
+# Degree split: the trace polynomials have degree D < 2n, so the weighted sum of the constraints of degree <= 2 of one zerofier
 # class has degree < 4n and is determined by its values on every second coset of the 8n-point quotient domain.  Those
-# constraints get their own ("lo") chunks; quotient.cu runs them on half of the rows and extends the four class sums with two
-# transforms per coordinate (exact: same field elements as evaluating everywhere).  25 % of the circuit's cost is in lo chunks.
+# constraints get their own ("lo") chunks.  When also 3D < 4n, quotient.cu runs the other chunks on half of the rows too and
+# corrects the class sums' part of degree >= 4n from the column tops (DESIGN.md section 3); the hi chunks that hold degree-4
+# constraints (CHUNK_DEGREE) run once more for that correction.  Exact: same field elements as evaluating everywhere.
 DEGREE_SPLIT = os.environ.get("TVM_AIR_DEGREE_SPLIT", "1") != "0"
 LOW_DEGREE = 2
 CHUNK_CLASS = {}   # chunk index -> "hi" | "lo" (filled by chunk_constraints)
+CHUNK_DEGREE = {}  # chunk index -> the largest degree of its constraints (filled by chunk_constraints)
 
 
 def mont(v):
@@ -146,6 +149,7 @@ def chunk_constraints(air, budget=None):
                     new_cost = sum(node_cost(b, x) for x in new) + 6.0
                     if cur and cost + new_cost > budget:
                         CHUNK_CLASS[len(chunks)] = cls
+                        CHUNK_DEGREE[len(chunks)] = max(b.degree(cs[i - offset]) for i, _ in cur)
                         chunks.append((cat, cur))
                         cur, seen, cost = [], set(), 0.0
                         new = [x for x in reachable_postorder(leaves) if x.kind in "+*"]
@@ -155,6 +159,7 @@ def chunk_constraints(air, budget=None):
                     cost += new_cost
             if cur:
                 CHUNK_CLASS[len(chunks)] = cls
+                CHUNK_DEGREE[len(chunks)] = max(b.degree(cs[i - offset]) for i, _ in cur)
                 chunks.append((cat, cur))
         offset += len(cs)
     return chunks
@@ -290,7 +295,7 @@ __global__ void __launch_bounds__(AIR_THREADS, %(minb)d) %(kname)s(AirArgs a) {
   const size_t n = (size_t)1 << a.log_n;
   const size_t coset = m >> a.log_n, k = m & (n - 1);
   const size_t mem_base = (coset * a.coset_mem_stride) << a.log_n;
-  const size_t m_cur = mem_base | k, m_next = mem_base | ((k + 1) & (n - 1));
+  const size_t m_cur = mem_base | k, m_next = a.next_offset ? m_cur + a.next_offset : mem_base | ((k + 1) & (n - 1));
   const u64 *mc = a.main + m_cur, *mn = a.main + m_next;
   const u64 *ac = a.aux + m_cur, *an = a.aux + m_next;
   (void)mn; (void)an; (void)ac; (void)mc; (void)coset;
@@ -304,15 +309,17 @@ static __device__ __noinline__ void %(bname)s(const u64 *mc, const u64 *mn, cons
 """
 
 TU_FOOTER = """
-// `lo`: the arguments of the chunks of constraints of degree <= 2 (see AirArgs::low_out); the same as `a` unless the caller splits
-void %(tuname)s_launch(const AirArgs &a, const AirArgs &lo, const u64 *d_wtab, const u64 *d_challenges, cudaStream_t s, unsigned long long *launches) {
+// `lo` / `hi`: the arguments of the chunks whose constraints have degree <= 2 / up to 4 (see AirArgs::low_out).  A chunk is
+// skipped when its group has no rows, or when its largest degree is below the group's min_degree.
+void %(tuname)s_launch(const AirArgs &lo, const AirArgs &hi, const u64 *d_wtab, const u64 *d_challenges, cudaStream_t s, unsigned long long *launches) {
   cudaMemcpyToSymbolAsync(c_w, d_wtab, sizeof(u64) * %(nw)d, 0, cudaMemcpyDeviceToDevice, s);
   cudaMemcpyToSymbolAsync(c_ch, d_challenges, sizeof(u64) * 189, 0, cudaMemcpyDeviceToDevice, s);
-  unsigned grid = (unsigned)((a.nrows + AIR_THREADS - 1) / AIR_THREADS);
-  unsigned grid_lo = (unsigned)((lo.nrows + AIR_THREADS - 1) / AIR_THREADS);
-  (void)grid_lo;
+  const unsigned grid_lo = (unsigned)((lo.nrows + AIR_THREADS - 1) / AIR_THREADS);
+  const unsigned grid_hi = (unsigned)((hi.nrows + AIR_THREADS - 1) / AIR_THREADS);
+  (void)grid_lo; (void)grid_hi;
+  unsigned long long nk = 0;
 %(launches)s
-  *launches += %(nk)d;
+  *launches += nk;
 }
 }  // namespace tvm
 """
@@ -341,19 +348,17 @@ def emit_body(air, idx, cat, items, fused):
 def emit_chunk(air, idx, cat, items):
     body, accs, nops = emit_body(air, idx, cat, items, False)
     low = CHUNK_CLASS.get(idx) == "lo"
+    deg = CHUNK_DEGREE[idx]
     kname = f"air_chunk_{idx:03d}_{cat}" + ("_lo" if low else "")
     if SYNC_EVERY:
         guard = "  const bool active = m < a.nrows;\n  if (!active) m = 0;   // keep every thread alive for the block-wide barriers below"
     else:
         guard = "  if (m >= a.nrows) return;\n  const bool active = true;"
-    src = [KERNEL_HEADER % {"kname": kname, "guard": guard, "minb": MIN_BLOCKS}]
+    src = [f"\n// constraints of degree <= {deg}" + KERNEL_HEADER % {"kname": kname, "guard": guard, "minb": MIN_BLOCKS}]
     src.append("  " + "\n  ".join(body))
     src.append("  AirAcc acc; air_acc_zero(acc);")
     src.extend("  " + x for x in accs)
-    if low:
-        src.append(f"  if (active) air_accumulate_low<{CATEGORIES.index(cat)}>(a, m, coset, air_acc_reduce(acc));")
-    else:
-        src.append(f"  if (active) air_accumulate_{cat}(a, m, coset, air_acc_reduce(acc));")
+    src.append(f"  if (active) air_accumulate_low<{CATEGORIES.index(cat)}>(a, m, coset, air_acc_reduce(acc));")
     src.append("}")
     return kname, "\n".join(src), nops
 
@@ -459,11 +464,10 @@ def main():
             names.append((kname, cat, ncons, nops))
             total_ops += nops
             parts.append(src)
-            if kname.endswith("_lo"):
-                launches.append(f"  {kname}<<<grid_lo, AIR_THREADS, 0, s>>>(lo);")
-            else:
-                launches.append(f"  {kname}<<<grid, AIR_THREADS, 0, s>>>(a);")
-        parts.append(TU_FOOTER % {"tuname": tuname, "nw": nw, "launches": "\n".join(launches), "nk": len(idxs)})
+            g = "lo" if kname.endswith("_lo") else "hi"
+            deg = 4 if FUSED else CHUNK_DEGREE[idx]
+            launches.append(f"  if ({g}.nrows && {g}.min_degree <= {deg}) {{ {kname}<<<grid_{g}, AIR_THREADS, 0, s>>>({g}); nk++; }}")
+        parts.append(TU_FOOTER % {"tuname": tuname, "nw": nw, "launches": "\n".join(launches)})
         with open(os.path.join(OUT_DIR, tuname + ".cu"), "w") as f:
             f.write("\n".join(parts))
     unique_ops = sum(sum(1 for n in reachable_postorder(air.constraints[c]) if n.kind in "+*") for c in CATEGORIES)

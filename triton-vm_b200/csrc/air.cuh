@@ -15,6 +15,7 @@ namespace tvm {
 static constexpr int AIR_THREADS = TVM_AIR_THREADS;
 static constexpr int AIR_MAX_COSETS = 64;
 
+static constexpr unsigned AIR_AUX_BCOLS = 270;   // aux B-field columns the constraints read (X-field columns 0..89)
 static constexpr int AIR_WTAB_WORDS = 7;   // per weight w = (b0,b1,b2): b0, b1, b2, -b1, -b2, b0+b2, b1-b2
 
 struct AirArgs {
@@ -22,6 +23,9 @@ struct AirArgs {
   size_t main_stride;
   const u64 *aux;       // aux X-field column q, coordinate d at aux + (3q+d)*aux_stride
   size_t aux_stride;
+  // 0: the "next row" is row (coset, k+1 mod n).  Otherwise it is read at the current row's index plus next_offset words in
+  // both tables (quotient.cu's top-degree correction stores the next-row polynomials as separate columns)
+  size_t next_offset;
   u64 *out;             // quotient codeword, planar: coordinate d at out + d*out_stride, memory order
   size_t out_stride;
   size_t nrows;         // (#cosets evaluated) * n
@@ -33,12 +37,12 @@ struct AirArgs {
   const u64 *zi_tran;   // (x - w_n^-1) / (x^n - 1)            (1216-1237)
   const u64 *zi_term;   // 1 / (x - w_n^-1)                    (1239-1252)
   u64 cons_zerofier_inv[AIR_MAX_COSETS];  // 1 / (x^n - 1), constant on a coset   (1204-1214)
-  // Degree split (quotient.cu): for tables that are low-degree extensions (degree < 2n), the weighted sum of the constraints
-  // of degree <= 2 of one zerofier class is a polynomial of degree < 4n.  The kernels of those constraints ("lo" chunks) then
-  // run on every second coset only and add their sums WITHOUT the zerofier inverse to low_out: class t (init, cons, tran,
-  // term), coordinate d at low_out + (3t + d) * low_stride, compact row index.  nullptr: they behave like all other chunks.
+  // Degree split (quotient.cu): the chunks given these arguments add their sums WITHOUT the zerofier inverse to low_out:
+  // class t (init, cons, tran, term), coordinate d at low_out + (3t + d) * low_stride, compact row index.  nullptr: they
+  // add the zerofier-weighted sums to `out`.
   u64 *low_out;
   size_t low_stride;
+  int min_degree;       // chunks whose constraints all have a smaller degree are not launched with these arguments
 };
 
 // strides handed to the chunk bodies of a fused group kernel (generated code refers to them as a.main_stride / a.aux_stride)

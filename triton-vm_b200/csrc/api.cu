@@ -1,6 +1,7 @@
 // extern "C" boundary of libtvm_b200 (kernel-level entry points).  See include/tvm_b200.h.
 #include "../../include/tvm_b200.h"
 #include "ctx.h"
+#include "air.cuh"
 #include "launch.h"
 #include "transcript.h"
 #include "prove_common.h"
@@ -450,6 +451,43 @@ int tvm_air_quotient_dev(tvm_ctx *ctx, const uint64_t *d_main, size_t main_strid
   TVM_CUDA(cudaStreamSynchronize(c__->stream));  // h is a stack-owned staging buffer
   air_quotient_run(*c__, (const u64 *)d_main, main_stride, (const u64 *)d_aux, aux_stride, d, d + nc, log2_trace, log2_cosets, 0, 1, 1u << log2_cosets, 1,
                    to_mont(offset_canon), (u64 *)d_out, out_stride);
+  TVM_API_END
+}
+
+int tvm_air_quotient_coef_dev(tvm_ctx *ctx, const uint64_t *d_main_coef, const uint64_t *d_aux_coef, size_t coef_stride,
+                              unsigned num_rand, const uint64_t *challenges, const uint64_t *weights, unsigned log2_trace,
+                              uint64_t offset_canon, uint64_t *d_out, size_t out_stride) {
+  if (!ctx || !d_main_coef || !d_aux_coef || !challenges || !weights || !d_out) return TVM_ERR_INVALID_ARG;
+  if (offset_canon == 0 || offset_canon >= P || log2_trace < 1 || log2_trace + 3 > 27) return TVM_ERR_DOMAIN;
+  const size_t n = (size_t)1 << log2_trace, len = n + num_rand;
+  if (num_rand > n || coef_stride < len || out_stride < 8 * n) return TVM_ERR_INVALID_ARG;
+  TVM_API_BEGIN(ctx)
+  Ctx &c = *c__;
+  const size_t nc = 3 * TVM_NUM_CHALLENGES, nw = 3 * TVM_NUM_CONSTRAINTS;
+  std::vector<u64> hw(nc + nw);
+  for (size_t i = 0; i < nc; i++) hw[i] = to_mont(challenges[i] % P);
+  for (size_t i = 0; i < nw; i++) hw[nc + i] = to_mont(weights[i] % P);
+  const size_t nmain = TVM_NUM_MAIN_COLUMNS, ncols = nmain + AIR_AUX_BCOLS, tmp_cols = 16;
+  // [consts | coefficients pre-scaled by offset^j [ncols][len] | LDE [ncols][8n] | transform scratch]
+  u64 *buf = (u64 *)c.pool_alloc(sizeof(u64) * (nc + nw + ncols * len + ncols * 8 * n + tmp_cols * 8 * n));
+  u64 *d = buf, *coef = d + nc + nw, *lde = coef + ncols * len, *tmp = lde + ncols * 8 * n;
+  try {
+    TVM_CUDA(cudaMemcpyAsync(d, hw.data(), (nc + nw) * 8, cudaMemcpyHostToDevice, c.stream));
+    TVM_CUDA(cudaMemcpy2DAsync(coef, len * 8, d_main_coef, coef_stride * 8, len * 8, nmain, cudaMemcpyDeviceToDevice, c.stream));
+    TVM_CUDA(cudaMemcpy2DAsync(coef + nmain * len, len * 8, d_aux_coef, coef_stride * 8, len * 8, AIR_AUX_BCOLS,
+                               cudaMemcpyDeviceToDevice, c.stream));
+    const u64 off = to_mont(offset_canon);
+    scale_by_powers_run(c, coef, len, (int)ncols, len, c.get_pow_tab(off, (int)log2_trace + 1));
+    for (size_t c0 = 0; c0 < ncols; c0 += tmp_cols)   // coefficients n..len-1 fold into 0..num_rand-1 (u^n = w_8^coset)
+      lde_evaluate_run(c, coef + c0 * len, len, num_rand, log2_trace, 3, 0, 1, 8, std::min(tmp_cols, ncols - c0), lde + c0 * 8 * n, tmp);
+    const AirCoefs cf{coef, coef + nmain * len, len, num_rand};
+    air_quotient_run(c, lde, 8 * n, lde + nmain * 8 * n, 8 * n, d, d + nc, log2_trace, 3, 0, 1, 8, 1, off, (u64 *)d_out, out_stride, &cf);
+    TVM_CUDA(cudaStreamSynchronize(c.stream));   // hw is a stack-owned staging buffer
+  } catch (...) {
+    c.pool_release(buf);
+    throw;
+  }
+  c.pool_release(buf);
   TVM_API_END
 }
 

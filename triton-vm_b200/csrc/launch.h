@@ -54,12 +54,20 @@ void merkle_run_sharded(Ctx &c, u64 *nodes, size_t nleaves, unsigned rank, unsig
 void xfe_leaves_run(Ctx &c, const u64 *cw, size_t stride, size_t n, u64 *leaves);
 void to_mont_run(Ctx &c, u64 *d, size_t n);
 void from_mont_run(Ctx &c, u64 *d, size_t n);
+// the tables of air_quotient_run as polynomials: pre-scaled interpolant coefficients (lde_interpolate_run), column q at
+// main + q*stride / aux + q*stride, of degree < n + num_rand
+struct AirCoefs {
+  const u64 *main, *aux;
+  size_t stride;
+  unsigned num_rand;
+};
 // evaluates on `num_cosets` of the 2^log_r cosets (domain coset coset_first + coset_step*y); the output holds only those
-// cosets ([y][k]); the tables hold coset y at memory coset y*coset_mem_stride ([col][..][k])
+// cosets ([y][k]); the tables hold coset y at memory coset y*coset_mem_stride ([col][..][k]).  `coefs` (optional) lets it
+// evaluate constraints on half of the domain (quotient.cu, the degree split)
 void air_quotient_run(Ctx &c, const u64 *d_main, size_t main_stride, const u64 *d_aux, size_t aux_stride,
                       const u64 *d_challenges, const u64 *d_weights, unsigned log_n, unsigned log_r,
                       unsigned coset_first, unsigned coset_step, unsigned num_cosets, unsigned coset_mem_stride,
-                      u64 offset_mont, u64 *d_out, size_t out_stride, bool low_degree_tables = false);   // see AirArgs::low_out
+                      u64 offset_mont, u64 *d_out, size_t out_stride, const AirCoefs *coefs = nullptr);
 // auxiliary-table extension (aux_extend.cu): d_main [379][n], d_ch [63*3], d_aux [273][n] planes, all Montgomery;
 // the batch-randomizer planes (column 90) are the caller's.  d_scratch: aux_extend_scratch_words(n) words
 size_t aux_extend_scratch_words(size_t n);

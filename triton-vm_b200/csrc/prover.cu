@@ -502,9 +502,10 @@ void stark_prove(Ctx &c, const StarkParams &sp, const ClaimView &claim, size_t p
     }
     mem.release(d_mc); mem.release(d_ac);
   } else {
-    // (the tables are low-degree extensions: with all cosets in one call the constraints of degree <= 2 run on half of them)
+    // (the tables' coefficients let the constraints run on half of the quotient domain when all of it is on this device)
+    const AirCoefs cf{d_main_coef, d_aux_coef, cs, (unsigned)h};
     air_quotient_run(c, d_main_lde, NLe, d_aux_lde, NLe, d_consts, d_consts + 3 * TVM_NUM_CHALLENGES, log_n, log_re, she.first, she.step * qs,
-                     she.count / qs, qs, off, d_quot + (size_t)rank * 3 * QL, QL, true);
+                     she.count / qs, qs, off, d_quot + (size_t)rank * 3 * QL, QL, W == 1 ? &cf : nullptr);
   }
   mark();  // 6: AIR quotient
 

@@ -228,6 +228,8 @@ _SIGNATURES = {
     "tvm_execution_destroy": (None, [_vp]),
     "tvm_air_quotient_dev": (ctypes.c_int, [_vp, _vp, ctypes.c_size_t, _vp, ctypes.c_size_t, _u64p, _u64p, ctypes.c_uint,
                                             ctypes.c_uint, ctypes.c_uint64, _vp, ctypes.c_size_t]),
+    "tvm_air_quotient_coef_dev": (ctypes.c_int, [_vp, _vp, _vp, ctypes.c_size_t, ctypes.c_uint, _u64p, _u64p, ctypes.c_uint,
+                                                 ctypes.c_uint64, _vp, ctypes.c_size_t]),
     "tvm_air_check": (ctypes.c_int, [_vp, _u64p, _u64p, ctypes.c_uint, _u64p, _u64p, _u64p, _u64p, _u64p]),
     "tvm_air_check_aet": (ctypes.c_int, [_vp, ctypes.POINTER(AetStruct), ctypes.POINTER(ClaimStruct), ctypes.c_uint64, _u64p, _u64p, _u64p,
                                          _u64p, _u64p]),
@@ -1002,6 +1004,14 @@ class Backend:
         assert ch.size == 189 and w.size == 1812
         self._chk(self._l.tvm_air_quotient_dev(self._h, self._dp(d_main), main_stride, self._dp(d_aux), aux_stride, chp, wp,
                                                log2_trace, log2_cosets, offset, self._dp(d_out), out_stride))
+
+    def air_quotient_coef_dev(self, d_main_coef, d_aux_coef, coef_stride, num_rand, challenges, weights, log2_trace, offset,
+                              d_out, out_stride):
+        ch, chp = _np_u64(np.asarray(challenges, dtype=np.uint64).reshape(-1))
+        w, wp = _np_u64(np.asarray(weights, dtype=np.uint64).reshape(-1))
+        assert ch.size == 189 and w.size == 1812
+        self._chk(self._l.tvm_air_quotient_coef_dev(self._h, self._dp(d_main_coef), self._dp(d_aux_coef), coef_stride, num_rand,
+                                                    chp, wp, log2_trace, offset, self._dp(d_out), out_stride))
 
     def merkle_dev(self, d_nodes, nleaves):
         self._chk(self._l.tvm_merkle_build_dev(self._h, self._dp(d_nodes), nleaves))
