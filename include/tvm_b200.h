@@ -97,6 +97,12 @@ int tvm_ntt_bfe(tvm_ctx *ctx, uint64_t *host_data, unsigned log2n, size_t ncols,
 int tvm_lde_bfe_dev(tvm_ctx *ctx, const uint64_t *d_trace, const uint64_t *d_rand, unsigned num_rand,
                     unsigned log2_trace, unsigned log2_cosets, uint64_t offset_canon, size_t ncols,
                     uint64_t *d_coef, uint64_t *d_out, uint64_t *d_tmp);
+/* the same on a subset of the r cosets, as one rank of a coset-sharded prove evaluates them: cosets
+ * c = coset_first + coset_step*y, y < num_cosets (all < r); d_out [ncols][num_cosets*n], d_out[q][y*n + k] */
+int tvm_lde_bfe_cosets_dev(tvm_ctx *ctx, const uint64_t *d_trace, const uint64_t *d_rand, unsigned num_rand,
+                           unsigned log2_trace, unsigned log2_cosets, uint64_t offset_canon, unsigned coset_first,
+                           unsigned coset_step, unsigned num_cosets, size_t ncols, uint64_t *d_coef, uint64_t *d_out,
+                           uint64_t *d_tmp);
 /* host buffers, canonical; out is [ncols][r*n] in NATURAL evaluation-domain order */
 int tvm_lde_bfe(tvm_ctx *ctx, const uint64_t *trace_colmajor, const uint64_t *rand, unsigned num_rand,
                 unsigned log2_trace, unsigned log2_cosets, uint64_t offset_canon, size_t ncols, uint64_t *out);

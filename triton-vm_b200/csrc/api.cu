@@ -331,6 +331,22 @@ int tvm_lde_bfe_dev(tvm_ctx *ctx, const uint64_t *d_trace, const uint64_t *d_ran
   TVM_API_END
 }
 
+int tvm_lde_bfe_cosets_dev(tvm_ctx *ctx, const uint64_t *d_trace, const uint64_t *d_rand, unsigned num_rand, unsigned log2_trace,
+                           unsigned log2_cosets, uint64_t offset_canon, unsigned coset_first, unsigned coset_step,
+                           unsigned num_cosets, size_t ncols, uint64_t *d_coef, uint64_t *d_out, uint64_t *d_tmp) {
+  if (!ctx || !d_trace || !d_coef || !d_out || !d_tmp) return TVM_ERR_INVALID_ARG;
+  if (log2_trace > 26 || log2_cosets > 6 || offset_canon >= P || offset_canon == 0) return TVM_ERR_DOMAIN;
+  if (num_cosets == 0 || coset_first + (uint64_t)coset_step * (num_cosets - 1) >= (1ull << log2_cosets)) return TVM_ERR_DOMAIN;
+  TVM_API_BEGIN(ctx)
+  if (!ncols) return TVM_OK;
+  const size_t n = (size_t)1 << log2_trace;
+  lde_interpolate_run(*c__, (const u64 *)d_trace, (const u64 *)d_rand, num_rand, num_rand, log2_trace, to_mont(offset_canon), ncols,
+                      (u64 *)d_coef, 2 * n, (u64 *)d_tmp);
+  lde_evaluate_run(*c__, (const u64 *)d_coef, 2 * n, d_rand ? num_rand : 0, log2_trace, log2_cosets, coset_first, coset_step, num_cosets,
+                   ncols, (u64 *)d_out, (u64 *)d_tmp);
+  TVM_API_END
+}
+
 int tvm_lde_bfe(tvm_ctx *ctx, const uint64_t *trace, const uint64_t *rand, unsigned num_rand, unsigned log2_trace,
                 unsigned log2_cosets, uint64_t offset_canon, size_t ncols, uint64_t *out) {
   if (!ctx || !trace || !out) return TVM_ERR_INVALID_ARG;

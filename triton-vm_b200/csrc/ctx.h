@@ -49,10 +49,14 @@ struct Ctx {
   int low_memory_mode = 0;              // 0 = automatic, 1 = always just-in-time LDE, 2 = never (tvm_ctx_set_low_memory)
   cudaStream_t copy_stream = nullptr;   // host<->device staging overlapped with compute (created on first use)
   std::vector<cudaEvent_t> copy_events; // recycled per-batch "upload done" events
-  // second compute stream of the tile NTT (ntt_tile.cu): alternate launch pairs fill each other's partial last waves
+  // second compute stream of the tile NTT's launch pairs (ntt_tile.cu, mixed radices): alternate pairs fill each other's
+  // partial last waves
   cudaStream_t pair_stream = nullptr;
   cudaEvent_t pair_fork = nullptr, pair_join = nullptr;
   cudaStream_t get_pair_stream();
+  // ticket and pair-completion counters of the persistent tile NTT (ntt_tile.cu), grown on demand
+  unsigned *tile_sync = nullptr;
+  size_t tile_sync_words = 0;
   cudaStream_t get_copy_stream();
   cudaEvent_t get_copy_event(size_t i);
   std::string last_error;

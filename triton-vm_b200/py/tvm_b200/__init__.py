@@ -178,6 +178,8 @@ _SIGNATURES = {
     "tvm_ntt_bfe": (ctypes.c_int, [_vp, _u64p, ctypes.c_uint, ctypes.c_size_t, ctypes.c_int]),
     "tvm_lde_bfe_dev": (ctypes.c_int, [_vp, _vp, _vp, ctypes.c_uint, ctypes.c_uint, ctypes.c_uint, ctypes.c_uint64,
                                        ctypes.c_size_t, _vp, _vp, _vp]),
+    "tvm_lde_bfe_cosets_dev": (ctypes.c_int, [_vp, _vp, _vp, ctypes.c_uint, ctypes.c_uint, ctypes.c_uint, ctypes.c_uint64,
+                                              ctypes.c_uint, ctypes.c_uint, ctypes.c_uint, ctypes.c_size_t, _vp, _vp, _vp]),
     "tvm_lde_bfe": (ctypes.c_int, [_vp, _u64p, _u64p, ctypes.c_uint, ctypes.c_uint, ctypes.c_uint, ctypes.c_uint64,
                                    ctypes.c_size_t, _u64p]),
     "tvm_tip5_hash_rows_dev": (ctypes.c_int, [_vp, _vp, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_uint, ctypes.c_uint, _vp]),
@@ -992,6 +994,12 @@ class Backend:
     def lde_dev(self, d_trace, d_rand, num_rand, log2_trace, log2_cosets, offset, ncols, d_coef, d_out, d_tmp):
         self._chk(self._l.tvm_lde_bfe_dev(self._h, self._dp(d_trace), self._dp(d_rand), num_rand, log2_trace, log2_cosets,
                                           offset, ncols, self._dp(d_coef), self._dp(d_out), self._dp(d_tmp)))
+
+    def lde_cosets_dev(self, d_trace, d_rand, num_rand, log2_trace, log2_cosets, offset, coset_first, coset_step, num_cosets,
+                       ncols, d_coef, d_out, d_tmp):
+        self._chk(self._l.tvm_lde_bfe_cosets_dev(self._h, self._dp(d_trace), self._dp(d_rand), num_rand, log2_trace, log2_cosets,
+                                                 offset, coset_first, coset_step, num_cosets, ncols, self._dp(d_coef),
+                                                 self._dp(d_out), self._dp(d_tmp)))
 
     def hash_rows_dev(self, d_table, col_stride, nrows, ncols, log2_cosets, d_digests):
         self._chk(self._l.tvm_tip5_hash_rows_dev(self._h, self._dp(d_table), col_stride, nrows, ncols, log2_cosets,
