@@ -49,6 +49,9 @@ int tvm_ctx_synchronize(tvm_ctx *ctx);
  * 2 = always cache.  The proof is identical in both modes. */
 int tvm_ctx_set_low_memory(tvm_ctx *ctx, int mode);
 int tvm_last_prove_low_memory(const tvm_ctx *ctx); /* 1 if the last tvm_prove ran just in time */
+/* Give the device memory the context keeps for reuse (blocks of earlier proves, scratch of the host-buffer entry points)
+ * back to the driver, after the context's stream has finished, so that other contexts and processes can use it. */
+int tvm_ctx_release_cached_memory(tvm_ctx *ctx);
 
 /* Multi-GPU: one process (and one context) per GPU.  A proof is sharded by evaluation-domain cosets
  * (SURVEY.md 8(e), mirroring the reference's own coset decomposition, stark.rs:824-885): rank g of

@@ -249,6 +249,24 @@ int tvm_ctx_set_low_memory(tvm_ctx *ctx, int mode) {
 }
 int tvm_last_prove_low_memory(const tvm_ctx *ctx) { return ctx && ctx->timings.low_memory ? 1 : 0; }
 
+int tvm_ctx_release_cached_memory(tvm_ctx *ctx) {
+  if (!ctx) return TVM_ERR_INVALID_ARG;
+  TVM_API_BEGIN(ctx)
+  TVM_CUDA(cudaStreamSynchronize(c__->stream));
+  while (!c__->pool_free.empty()) {         // each block leaves the pool before it is freed: no double free on an error
+    void *p = c__->pool_free.begin()->second;
+    c__->pool_free.erase(c__->pool_free.begin());
+    TVM_CUDA(cudaFree(p));
+  }
+  for (auto &s : c__->scratch) {
+    void *p = s.p;
+    s.p = nullptr;
+    s.bytes = 0;
+    if (p) TVM_CUDA(cudaFree(p));
+  }
+  TVM_API_END
+}
+
 int tvm_ctx_synchronize(tvm_ctx *ctx) {
   if (!ctx) return TVM_ERR_INVALID_ARG;
   TVM_API_BEGIN(ctx)

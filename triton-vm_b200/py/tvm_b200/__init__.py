@@ -168,6 +168,7 @@ _SIGNATURES = {
     "tvm_ctx_set_comm": (ctypes.c_int, [_vp, ctypes.POINTER(CommStruct)]),
     "tvm_ctx_set_low_memory": (ctypes.c_int, [_vp, ctypes.c_int]),
     "tvm_last_prove_low_memory": (ctypes.c_int, [_vp]),
+    "tvm_ctx_release_cached_memory": (ctypes.c_int, [_vp]),
     "tvm_strerror": (ctypes.c_char_p, [ctypes.c_int]),
     "tvm_last_error": (ctypes.c_char_p, [_vp]),
     "tvm_launch_count": (ctypes.c_uint64, [_vp]),
@@ -957,6 +958,10 @@ class Backend:
     @property
     def last_prove_low_memory(self):
         return bool(self._l.tvm_last_prove_low_memory(self._h))
+
+    def release_cached_memory(self):
+        """tvm_ctx_release_cached_memory: the device memory this context keeps for reuse goes back to the driver"""
+        self._chk(self._l.tvm_ctx_release_cached_memory(self._h))
 
     def set_comm(self, comm):
         """Attach a communication layer (tvm_b200.dist.TorchDistComm) so that prove() shards one proof over
