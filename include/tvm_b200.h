@@ -12,8 +12,10 @@
  *    (R = 2^64; twenty-first's in-memory representation) and never touch host memory.
  *  - All functions return 0 on success or a negative TVM_ERR_* code; no exceptions or panics
  *    cross the ABI.  tvm_last_error() gives a human-readable description.
- *  - A tvm_ctx is single-caller (like the reference's prove(): one driving thread); several
- *    contexts may run concurrently on different devices.
+ *  - A tvm_ctx is single-caller (like the reference's prove(): one driving thread at a time).
+ *    Several contexts may run concurrently, each from its own thread, on different devices or on
+ *    the same one: their stages overlap on the GPU, except the AIR constraint evaluation
+ *    (quotient and check), which takes the device's constant banks in turn.
  *  - Caller owns every host pointer, for the duration of the call only.
  */
 #ifndef TVM_B200_H

@@ -107,10 +107,13 @@ void air_check_run(Ctx &c, DevMem &mem, const u64 *d_main, const u64 *d_aux, siz
   args[1].nrows = n;                                      // cons: every row
   args[2].nrows = n - 1;                                  // tran: (i, i+1) for i < n - 1
   args[3].first_row = n - 1; args[3].nrows = 1;           // term: row n - 1
+  {
+    AirConstLease lease(c);   // each translation unit uploads the challenges into its constant bank, shared by the device
 #define TVM_AIR_CHECK_TU(tu) tu##_launch(args, d, c.stream, &c.launches);
 #include "air_check_gen/air_check_meta.inc"
 #undef TVM_AIR_CHECK_TU
-  TVM_CUDA(cudaGetLastError());
+    TVM_CUDA(cudaGetLastError());
+  }
   const std::vector<u64> out = d2h(c, d + nch, 3 * NC);   // synchronises: `h` may go
   uint64_t violated = 0;
   for (size_t j = 0; j < NC; j++) {

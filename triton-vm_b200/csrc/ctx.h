@@ -4,6 +4,7 @@
 #include <cstdio>
 #include <functional>
 #include <map>
+#include <mutex>
 #include <string>
 #include <tuple>
 #include <vector>
@@ -86,6 +87,24 @@ struct Ctx {
   void *scratch_get(int slot, size_t bytes);
   const u64 *get_tile_tw(int LT, bool inverse);
   PowTab get_pow_tab(u64 base_mont, int log_count);  // exponents < 2^log_count
+};
+
+// Exclusive use of the device's AIR constant banks.  The generated AIR kernels (air_gen/, air_check_gen/) read the weights
+// and challenges from __constant__ memory, which every context on a device shares, and their launch functions upload it on
+// the caller's stream.  A lease holds the device's process-wide mutex and makes c.stream wait for the previous owner's last
+// AIR work (an event recorded when that lease ended); its destructor records the event on c.stream and unlocks, on an
+// exception too.  The mutex is held only while work is enqueued (DESIGN.md §6j: why that cannot deadlock).
+class AirConstLease {
+ public:
+  explicit AirConstLease(Ctx &c);
+  ~AirConstLease();
+  AirConstLease(const AirConstLease &) = delete;
+  AirConstLease &operator=(const AirConstLease &) = delete;
+
+ private:
+  Ctx &c_;
+  std::unique_lock<std::mutex> lock_;
+  cudaEvent_t last_use_ = nullptr;
 };
 
 u64 root_of_unity_mont(unsigned log2n);  // twenty-first's PRIMITIVE_ROOTS, Montgomery form

@@ -389,9 +389,20 @@ static size_t tile_smem_bytes(int LT, int log_t) {
   return (N + ((N + 2) << log_t)) * sizeof(u64);
 }
 
+// The dynamic shared-memory limit is an attribute of the kernel on a device, shared by every context of the process, and these
+// kernels launch with a size that depends on the transform.  So the limit only ever grows: setting it to this launch's size
+// could lower it between another context's set and launch, and that launch would fail with cudaErrorInvalidValue.
 template <class K>
 static void set_smem(K kernel, size_t bytes) {
+  static std::mutex m;
+  static auto *limits = new std::map<std::pair<int, const void *>, size_t>();   // (device, kernel) -> limit set; never destroyed
+  int dev = 0;
+  TVM_CUDA(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> g(m);
+  size_t &limit = (*limits)[{dev, (const void *)kernel}];
+  if (bytes <= limit) return;
   TVM_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  limit = bytes;
 }
 
 void ntt_run(Ctx &c, const NttJob &job) {

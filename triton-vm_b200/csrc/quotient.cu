@@ -13,6 +13,30 @@ namespace tvm {
 #include "air_gen/air_chunks.inc"
 #undef TVM_AIR_TU
 
+namespace {
+struct AirConstSlot {
+  std::mutex m;
+  cudaEvent_t last_use = nullptr;   // recorded at the end of every lease on this device (created by the first one)
+};
+AirConstSlot &air_const_slot(int device) {
+  static std::mutex registry;
+  static auto *slots = new std::map<int, AirConstSlot>();   // never destroyed: a context may outlive static destruction
+  std::lock_guard<std::mutex> g(registry);
+  return (*slots)[device];
+}
+}  // namespace
+
+AirConstLease::AirConstLease(Ctx &c) : c_(c) {
+  AirConstSlot &s = air_const_slot(c.device);
+  std::unique_lock<std::mutex> lock(s.m);
+  if (!s.last_use) TVM_CUDA(cudaEventCreateWithFlags(&s.last_use, cudaEventDisableTiming));
+  TVM_CUDA(cudaStreamWaitEvent(c.stream, s.last_use, 0));
+  last_use_ = s.last_use;
+  lock_ = std::move(lock);
+}
+
+AirConstLease::~AirConstLease() { cudaEventRecord(last_use_, c_.stream); }
+
 // weight table: 7 words per weight (air.cuh, AIR_WTAB_WORDS)
 __global__ void air_weight_table_kernel(const u64 *w, unsigned count, u64 *tab) {
   unsigned j = blockIdx.x * blockDim.x + threadIdx.x;
@@ -203,6 +227,8 @@ void air_quotient_run(Ctx &c, const u64 *d_main, size_t main_stride, const u64 *
                       unsigned coset_first, unsigned coset_step, unsigned num_cosets, unsigned coset_mem_stride,
                       u64 offset_mont, u64 *d_out, size_t out_stride, const AirCoefs *coefs) {
   if (num_cosets > (unsigned)AIR_MAX_COSETS) throw ApiError{TVM_ERR_UNSUPPORTED, "too many cosets"};
+  // every chunk launch below (air_top_correction's too) uploads and reads the device's constant banks
+  AirConstLease lease(c);
   // The degree split needs the whole domain in one call, at least 8n points of it, and the tables' degree D = n + h - 1
   // (known from their coefficients).  Constraints of degree <= 2 run on the even cosets when 2D < 4n (their class sums have
   // degree < 4n); all of them do when in addition 3D < 4n on exactly 8n points (air_top_correction).

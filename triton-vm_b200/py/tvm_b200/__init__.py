@@ -523,7 +523,9 @@ def proof_padded_height(proof):
 
 
 class Backend:
-    """One context = one GPU = one driving thread (mirrors Prover::prove being single-caller)."""
+    """One context on one GPU, driven by one thread at a time (mirrors Prover::prove being single-caller).  Several Backends
+    may work concurrently, also on the same GPU, each from its own thread: the library is loaded with ctypes.CDLL, so every
+    call releases the GIL for its whole duration (a prove's aux_provider callback takes it back while it runs)."""
 
     def __init__(self, device=0):
         self._l = lib()
