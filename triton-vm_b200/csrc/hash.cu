@@ -6,12 +6,10 @@
 // node 2i+1), root = node 1, leaf j = node n + j (SURVEY.md A.4).  FRI codeword trees use the
 // unhashed leaf Digest::from(xfe) = (c0,c1,c2,0,0) (fri.rs:343-347, 927-929).
 //
-// Mapping: one thread per row with the 16-lane sponge state resident in registers for the
-// whole absorb loop (all 5 rounds fused; no state traffic), tables stored column-major so that
-// a warp's loads of one column are a single coalesced 256-byte segment.  The S-box lookup table
-// lives in shared memory; the round constants in constant memory (warp-uniform index).
+// Mapping: rows and inner nodes go through the IMMA permutation, four lanes per state and two states
+// per lane quad.  Thread-per-node kernels (the whole state in one thread's registers) handle Merkle
+// levels narrower than 64 nodes and the top of the tree.
 #include <cstdint>
-#include <cstdlib>
 #include "ctx.h"
 #include "tip5.cuh"
 #include "tip5_constants.inc"
@@ -48,40 +46,6 @@ struct HashRowsParams {
   u64 *digests;         // [nrows][5], natural row order
   unsigned coset_mem_stride;   // rows of coset c are read from table coset c * coset_mem_stride
 };
-
-__global__ void __launch_bounds__(HASH_THREADS) tip5_hash_rows_kernel(HashRowsParams p) {
-  __shared__ unsigned char lut[256];
-  for (int i = threadIdx.x; i < 256; i += blockDim.x) lut[i] = c_tip5_lut[i];
-  __syncthreads();
-  size_t m = (size_t)blockIdx.x * blockDim.x + threadIdx.x;  // memory-order index within a column
-  if (m >= p.nrows) return;
-  // memory index m = coset * (nrows >> log_r) + k  <->  row i = coset + (k << log_r)
-  size_t per = p.nrows >> p.log_r;
-  size_t coset = m / per, k = m - coset * per;
-  size_t row = coset + (k << p.log_r);
-  const u64 *base = p.table + m;
-  u64 s[16];
-#pragma unroll
-  for (int i = 0; i < 16; i++) s[i] = 0;
-  unsigned c = 0;
-  for (; c + 10 <= p.ncols; c += 10) {
-#pragma unroll
-    for (int i = 0; i < 10; i++) s[i] = base[(size_t)(c + i) * p.col_stride];
-    tip5_perm_dev(s, lut);
-  }
-  unsigned rem = p.ncols - c;
-#pragma unroll
-  for (int i = 0; i < 10; i++) {
-    u64 v = 0;
-    if ((unsigned)i < rem) v = base[(size_t)(c + i) * p.col_stride];
-    else if ((unsigned)i == rem) v = MONT_ONE;
-    s[i] = v;
-  }
-  tip5_perm_dev(s, lut);
-  u64 *d = p.digests + row * 5;
-#pragma unroll
-  for (int i = 0; i < 5; i++) d[i] = s[i];
-}
 
 // nodes: [2*nleaves][5]; computes nodes[lo .. lo+count) from their children.
 __global__ void __launch_bounds__(HASH_THREADS) merkle_level_kernel(u64 *nodes, size_t lo, size_t count) {
@@ -134,67 +98,9 @@ __global__ void xfe_leaves_kernel(const u64 *cw, size_t stride, size_t n, u64 *l
   d[0] = cw[i]; d[1] = cw[stride + i]; d[2] = cw[2 * stride + i]; d[3] = 0; d[4] = 0;
 }
 
-
-// ---- warp-resident variant: 4 lanes per row ---------------------------------------------------
-// Lane l of a 4-lane group holds state elements {l, l+4, l+8, l+12}: every lane has one
-// split-and-lookup element (slot 0) and three x^7 elements, so the S-box layer is divergence-free.
-// The circulant MDS product gathers the 16 inputs by warp shuffle in a lane-rotated order
-// (X[k] = x_{(k+l) mod 16}), which makes the matrix constants identical for all lanes
-// (y_{l+4i} = sum_k M[(4i-k) mod 16] X[k]).  Compared with one thread per row this keeps the round
-// body ~4x smaller (instruction-cache resident) and the register count low (more resident warps).
-__device__ __forceinline__ u64 shfl64(u64 v, int src) {
-  unsigned lo = __shfl_sync(0xffffffffu, (unsigned)v, src);
-  unsigned hi = __shfl_sync(0xffffffffu, (unsigned)(v >> 32), src);
-  return ((u64)hi << 32) | lo;
-}
-
-__device__ __forceinline__ void tip5_perm_quad(u64 (&s)[4], int l, int group_base, const unsigned char *lut, const u64 *rc_smem) {
-  constexpr unsigned short MDS[16] = TVM_MDS_COL;
-#pragma unroll 1
-  for (int rnd = 0; rnd < TIP5_ROUNDS; rnd++) {
-    {  // slot 0: split-and-lookup
-      u64 v = s[0], o = 0;
-#pragma unroll
-      for (int b = 0; b < 8; b++) o |= (u64)lut[(unsigned)((v >> (8 * b)) & 0xFF)] << (8 * b);
-      s[0] = o;
-    }
-#pragma unroll
-    for (int i = 1; i < 4; i++) {
-      u64 x = s[i], x2 = fmul(x, x), x3 = fmul(x2, x), x4 = fmul(x2, x2);
-      s[i] = fmul(x3, x4);
-    }
-    u64 lo[4] = {0, 0, 0, 0}, hi[4] = {0, 0, 0, 0};
-#pragma unroll
-    for (int k = 0; k < 16; k++) {
-      // this lane provides, to the lane l' that wants element (k + l') mod 16 with (k + l') mod 4 == l,
-      // its slot ((k + ((l - k) & 3)) & 15) >> 2
-      const int wrap = (((l - k) & 3) + (k & 3)) >> 2;          // 0 or 1
-      const u64 provide = wrap ? s[((k >> 2) + 1) & 3] : s[k >> 2];
-      const u64 X = shfl64(provide, group_base + ((k + l) & 3));
-      const u64 xl = X & 0xFFFFFFFFULL, xh = X >> 32;
-#pragma unroll
-      for (int i = 0; i < 4; i++) {
-        const u64 m = MDS[(4 * i - k) & 15];
-        lo[i] += m * xl;
-        hi[i] += m * xh;
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-      u64 lsum = lo[i] + (hi[i] << 32);
-      u64 carry = lsum < lo[i];
-      u64 h = (hi[i] >> 32) + carry;
-      s[i] = fadd(reduce96(lsum, h), rc_smem[16 * rnd + l + 4 * i]);
-    }
-  }
-}
-
-// ---- two rows per lane quad ---------------------------------------------------------------------
-// The round of one state is a long FMA-pipe stretch (MDS: 128 IMAD.WIDE per lane) followed by
-// ALU-pipe stretches (reductions, S-box bookkeeping); with every warp of an SM running the same
-// stream the two pipes are used alternately rather than concurrently (ncu r01b: issue 54 %,
-// `math_pipe_throttle` the top stall).  Each quad therefore carries two independent rows, half a
-// round out of phase: the MDS of one state is scheduled together with the S-box of the other.
+// ---- four lanes per state, two states per lane quad ---------------------------------------------
+// Lane l of a quad holds elements {l, l+4, l+8, l+12} of each of its two states: slot 0 is a
+// split-and-lookup element and slots 1..3 take x^7, so quad_sbox is divergence-free.
 // split-and-lookup (tip-0005.md:52-61) of one 32-bit half: byte extraction and re-assembly with PRMT (the shift/mask/or
 // form costs ~6 instructions per byte, this one 11 per four bytes); the looked-up values are zero-extended bytes, so
 // "byte 1 of l" is a zero for the unused selector positions
@@ -215,158 +121,6 @@ __device__ __forceinline__ void quad_sbox(u64 (&s)[4], const unsigned char *lut)
 #pragma unroll
   for (int i = 1; i < 4; i++) s[i] = pow7(s[i]);
 }
-__device__ __forceinline__ void quad_mds_rc(u64 (&s)[4], int l, int group_base, const u64 *rc_smem, int rnd) {
-  constexpr unsigned short MDS[16] = TVM_MDS_COL;
-  u64 lo[4] = {0, 0, 0, 0}, hi[4] = {0, 0, 0, 0};
-#pragma unroll
-  for (int k = 0; k < 16; k++) {
-    const int wrap = (((l - k) & 3) + (k & 3)) >> 2;          // 0 or 1
-    const u64 provide = wrap ? s[((k >> 2) + 1) & 3] : s[k >> 2];
-    const u64 X = shfl64(provide, group_base + ((k + l) & 3));
-    const u64 xl = X & 0xFFFFFFFFULL, xh = X >> 32;
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-      const u64 m = MDS[(4 * i - k) & 15];
-      lo[i] += m * xl;
-      hi[i] += m * xh;
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < 4; i++) {
-    u64 lsum = lo[i] + (hi[i] << 32);
-    u64 carry = lsum < lo[i];
-    u64 h = (hi[i] >> 32) + carry;
-    s[i] = fadd(reduce96(lsum, h), rc_smem[16 * rnd + l + 4 * i]);
-  }
-}
-// Same MDS step with the 16 inputs exchanged through shared memory instead of 32 shuffles + 32 selects (cost model:
-// SHFL 4 clocks, SEL 2; LDS.64 ~2): the quad writes its state to a 20-word-strided slot (bank-conflict free: word index
-// 20*s + e covers all 16 residues mod 16 for 4 consecutive quads, two wavefronts per 64-bit warp access) and every
-// lane reads x_{(k+l) mod 16}.
-static constexpr int XCH_STRIDE = 20;
-__device__ __forceinline__ void quad_mds_rc_smem(u64 (&s)[4], int l, u64 *slot, const u64 *rc_smem, int rnd) {
-  constexpr unsigned short MDS[16] = TVM_MDS_COL;
-  __syncwarp();                                   // previous readers of this slot are done
-#pragma unroll
-  for (int i = 0; i < 4; i++) slot[l + 4 * i] = s[i];
-  __syncwarp();
-  u64 lo[4] = {0, 0, 0, 0}, hi[4] = {0, 0, 0, 0};
-#pragma unroll
-  for (int k = 0; k < 16; k++) {
-    const u64 X = slot[(k + l) & 15];
-    const u64 xl = X & 0xFFFFFFFFULL, xh = X >> 32;
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-      const u64 m = MDS[(4 * i - k) & 15];
-      lo[i] += m * xl;
-      hi[i] += m * xh;
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < 4; i++) {
-    u64 lsum = lo[i] + (hi[i] << 32);
-    u64 carry = lsum < lo[i];
-    u64 h = (hi[i] >> 32) + carry;
-    s[i] = fadd(reduce96(lsum, h), rc_smem[16 * rnd + l + 4 * i]);
-  }
-}
-template <bool SMEM>
-__device__ __forceinline__ void quad_mds_sel(u64 (&s)[4], int l, int group_base, u64 *slot, const u64 *rc_smem, int rnd) {
-  if (SMEM) quad_mds_rc_smem(s, l, slot, rc_smem, rnd);
-  else quad_mds_rc(s, l, group_base, rc_smem, rnd);
-}
-template <bool SMEM>
-__device__ __forceinline__ void tip5_perm_quad2x(u64 (&a)[4], u64 (&b)[4], int l, int group_base, const unsigned char *lut,
-                                                 const u64 *rc_smem, u64 *slot_a, u64 *slot_b) {
-  quad_sbox(a, lut);
-#pragma unroll 1
-  for (int rnd = 0; rnd < TIP5_ROUNDS - 1; rnd++) {
-    quad_mds_sel<SMEM>(a, l, group_base, slot_a, rc_smem, rnd);
-    quad_sbox(b, lut);
-    quad_mds_sel<SMEM>(b, l, group_base, slot_b, rc_smem, rnd);
-    quad_sbox(a, lut);
-  }
-  quad_mds_sel<SMEM>(a, l, group_base, slot_a, rc_smem, TIP5_ROUNDS - 1);
-  quad_sbox(b, lut);
-  quad_mds_sel<SMEM>(b, l, group_base, slot_b, rc_smem, TIP5_ROUNDS - 1);
-}
-__device__ __forceinline__ void tip5_perm_quad2(u64 (&a)[4], u64 (&b)[4], int l, int group_base, const unsigned char *lut,
-                                                const u64 *rc_smem) {
-  quad_sbox(a, lut);
-#pragma unroll 1
-  for (int rnd = 0; rnd < TIP5_ROUNDS - 1; rnd++) {
-    quad_mds_rc(a, l, group_base, rc_smem, rnd);
-    quad_sbox(b, lut);
-    quad_mds_rc(b, l, group_base, rc_smem, rnd);
-    quad_sbox(a, lut);
-  }
-  quad_mds_rc(a, l, group_base, rc_smem, TIP5_ROUNDS - 1);
-  quad_sbox(b, lut);
-  quad_mds_rc(b, l, group_base, rc_smem, TIP5_ROUNDS - 1);
-}
-
-static constexpr int HASHQ2_THREADS = 128;   // 32 quads, 64 rows per CTA
-template <bool SMEM>
-__global__ void __launch_bounds__(HASHQ2_THREADS) tip5_hash_rows_quad2_kernel(HashRowsParams p) {
-  __shared__ unsigned char lut[256];
-  __shared__ u64 rc[80];
-  __shared__ u64 xch[SMEM ? 2 * (HASHQ2_THREADS / 4) * XCH_STRIDE : 1];
-  u64 *slot_a = xch + (SMEM ? (threadIdx.x >> 2) * XCH_STRIDE : 0);
-  u64 *slot_b = xch + (SMEM ? ((HASHQ2_THREADS / 4) + (threadIdx.x >> 2)) * XCH_STRIDE : 0);
-  for (int i = threadIdx.x; i < 256; i += blockDim.x) lut[i] = c_tip5_lut[i];
-  for (int i = threadIdx.x; i < 80; i += blockDim.x) rc[i] = c_tip5_rc[i];
-  __syncthreads();
-  const int lane = threadIdx.x & 31, l = lane & 3, group_base = lane & ~3;
-  constexpr int QUADS = HASHQ2_THREADS / 4;
-  size_t mrow[2];
-  bool active[2];
-  const u64 *base[2];
-#pragma unroll
-  for (int t = 0; t < 2; t++) {
-    size_t m = (size_t)blockIdx.x * (2 * QUADS) + (threadIdx.x >> 2) + (size_t)t * QUADS;
-    active[t] = m < p.nrows;
-    if (!active[t]) m = p.nrows - 1;                              // keep the quad alive for the shuffles
-    mrow[t] = m;
-    const size_t per_ = p.nrows >> p.log_r, cs_ = m / per_;
-    base[t] = p.table + m + cs_ * (p.coset_mem_stride - 1) * per_;
-  }
-  u64 a[4] = {0, 0, 0, 0}, b[4] = {0, 0, 0, 0};
-  unsigned c = 0;
-  for (; c + 10 <= p.ncols; c += 10) {
-    a[0] = base[0][(size_t)(c + l) * p.col_stride];
-    b[0] = base[1][(size_t)(c + l) * p.col_stride];
-    a[1] = base[0][(size_t)(c + l + 4) * p.col_stride];
-    b[1] = base[1][(size_t)(c + l + 4) * p.col_stride];
-    if (l < 2) {
-      a[2] = base[0][(size_t)(c + l + 8) * p.col_stride];
-      b[2] = base[1][(size_t)(c + l + 8) * p.col_stride];
-    }
-    tip5_perm_quad2x<SMEM>(a, b, l, group_base, lut, rc, slot_a, slot_b);
-  }
-  unsigned rem = p.ncols - c;
-#pragma unroll
-  for (int i = 0; i < 3; i++) {
-    unsigned e = (unsigned)(l + 4 * i);
-    if (e < 10) {
-      u64 va = 0, vb = 0;
-      if (e < rem) { va = base[0][(size_t)(c + e) * p.col_stride]; vb = base[1][(size_t)(c + e) * p.col_stride]; }
-      else if (e == rem) { va = MONT_ONE; vb = MONT_ONE; }
-      a[i] = va; b[i] = vb;
-    }
-  }
-  tip5_perm_quad2x<SMEM>(a, b, l, group_base, lut, rc, slot_a, slot_b);
-  const size_t per = p.nrows >> p.log_r;
-#pragma unroll
-  for (int t = 0; t < 2; t++) {
-    if (!active[t]) continue;
-    size_t m = mrow[t];
-    size_t coset = m / per, k = m - coset * per;
-    u64 *d = p.digests + (coset + (k << p.log_r)) * 5;
-    const u64 *s = t ? b : a;
-    d[l] = s[0];
-    if (l == 0) d[4] = s[1];
-  }
-}
 
 // ---- MDS on the tensor cores: IMMA.16832.U8.U8 -----------------------------------------------------
 // The linear layer y = M x (tip-0005.md:100-104) is a dense 16x16 integer matrix product applied to every state:
@@ -374,7 +128,7 @@ __global__ void __launch_bounds__(HASHQ2_THREADS) tip5_hash_rows_quad2_kernel(Ha
 // byte limbs  x_e = sum_s 2^(8s) X_s[e],  M = M_0 + 2^8 M_1  the product is
 //     y_o = sum_{s=0..8} 2^(8s) T_s[o],      T_s = M_0 X_s + M_1 X_{s-1}      (X_{-1} = X_8 = 0, T_s < 2^21),
 // and T_s for 16 states x 8 outputs is exactly one mma.sync.m16n8k32 (u8 x u8 -> s32): K = 32 = 16 state elements x
-// {limb s against M_0, limb s-1 against M_1}.  Layout: the quad layout of the kernels above with two rows per quad
+// {limb s against M_0, limb s-1 against M_1}.  Layout: the quad layout above with two rows per quad
 // IS the IMMA A-fragment layout (fragment row g / g+8 = first / second row of quad g, fragment k = 4l+t = element
 // l+4t of lane l), and choosing the B-fragment column order as o(j, n) = (n >> 1) + 4 (2j + (n & 1)) makes the
 // D fragment of N-block j land on the lane that owns the output element: c0/c1 = elements l+8j, l+8j+4 of the first row,
@@ -769,195 +523,22 @@ __global__ void __launch_bounds__(HASHM_THREADS) merkle_level_mma_kernel(u64 *no
   }
 }
 
-// ---- two lanes per row ------------------------------------------------------------------------------
-// Measured cost model (tools/microbench/field_ops.cu, SMSP-clocks per warp instruction group): the MDS step
-// of the 4-lane layout costs 635 per round against 355 for the three x^7 - its 32 shuffles (4 clocks
-// each) and 32 selects are paid by every lane for a quarter of a state.  With two lanes per row, lane l
-// holding elements {l, l+2, ..., l+14} (slots 0,1 = split-and-lookup, slots 2..7 = x^7, again
-// divergence-free), the rotated gather X[k] = x_{(k+l) mod 16} needs the partner only for odd k:
-// 16 shuffles + 16 selects per lane for HALF a state, and the IMAD count per state is unchanged.
-__device__ __forceinline__ void pair_sbox(u64 (&s)[8], const unsigned char *lut) {
-#pragma unroll
-  for (int j = 0; j < 2; j++) {
-    u64 v = s[j], o = 0;
-#pragma unroll
-    for (int b = 0; b < 8; b++) o |= (u64)lut[(unsigned)((v >> (8 * b)) & 0xFF)] << (8 * b);
-    s[j] = o;
-  }
-#pragma unroll
-  for (int j = 2; j < 8; j++) {
-    u64 x = s[j], x2 = fmul(x, x), x3 = fmul(x2, x), x4 = fmul(x2, x2);
-    s[j] = fmul(x3, x4);
-  }
-}
-__device__ __forceinline__ void pair_mds_rc(u64 (&s)[8], int l, const u64 *rc_smem, int rnd) {
-  constexpr unsigned short MDS[16] = TVM_MDS_COL;
-  u64 lo[8], hi[8];
-#pragma unroll
-  for (int i = 0; i < 8; i++) { lo[i] = 0; hi[i] = 0; }
-#pragma unroll
-  for (int k = 0; k < 16; k++) {
-    u64 X;
-    if ((k & 1) == 0) {
-      X = s[k >> 1];                                           // own element k + l
-    } else {
-      // the partner wants x_{(k + l') mod 16}: lane 1 serves lane 0 with slot (k-1)/2, lane 0 serves lane 1
-      // with slot ((k+1) mod 16)/2
-      const u64 provide = l ? s[(k - 1) >> 1] : s[((k + 1) & 15) >> 1];
-      unsigned plo = __shfl_xor_sync(0xffffffffu, (unsigned)provide, 1);
-      unsigned phi = __shfl_xor_sync(0xffffffffu, (unsigned)(provide >> 32), 1);
-      X = ((u64)phi << 32) | plo;
-    }
-    const u64 xl = X & 0xFFFFFFFFULL, xh = X >> 32;
-#pragma unroll
-    for (int i = 0; i < 8; i++) {
-      const u64 m = MDS[(2 * i - k) & 15];
-      lo[i] += m * xl;
-      hi[i] += m * xh;
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < 8; i++) {
-    u64 lsum = lo[i] + (hi[i] << 32);
-    u64 carry = lsum < lo[i];
-    u64 h = (hi[i] >> 32) + carry;
-    s[i] = fadd(reduce96(lsum, h), rc_smem[16 * rnd + l + 2 * i]);
-  }
-}
-__device__ __forceinline__ void tip5_perm_pair(u64 (&s)[8], int l, const unsigned char *lut, const u64 *rc_smem) {
-#pragma unroll 1
-  for (int rnd = 0; rnd < TIP5_ROUNDS; rnd++) {
-    pair_sbox(s, lut);
-    pair_mds_rc(s, l, rc_smem, rnd);
-  }
-}
-
-static constexpr int HASHP_THREADS = 128;    // 64 rows per CTA
-__global__ void __launch_bounds__(HASHP_THREADS) tip5_hash_rows_pair_kernel(HashRowsParams p) {
-  __shared__ unsigned char lut[256];
-  __shared__ u64 rc[80];
-  for (int i = threadIdx.x; i < 256; i += blockDim.x) lut[i] = c_tip5_lut[i];
-  for (int i = threadIdx.x; i < 80; i += blockDim.x) rc[i] = c_tip5_rc[i];
-  __syncthreads();
-  const int l = threadIdx.x & 1;
-  size_t m = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 1;   // one row per 2 lanes
-  const bool active = m < p.nrows;
-  if (!active) m = p.nrows - 1;                                     // keep the pair alive for the shuffles
-  const u64 *base = p.table + m;
-  u64 s[8];
-#pragma unroll
-  for (int j = 0; j < 8; j++) s[j] = 0;
-  unsigned c = 0;
-  for (; c + 10 <= p.ncols; c += 10) {
-#pragma unroll
-    for (int j = 0; j < 5; j++) s[j] = base[(size_t)(c + l + 2 * j) * p.col_stride];
-    tip5_perm_pair(s, l, lut, rc);
-  }
-  const unsigned rem = p.ncols - c;
-#pragma unroll
-  for (int j = 0; j < 5; j++) {
-    const unsigned e = (unsigned)(l + 2 * j);
-    u64 v = 0;
-    if (e < rem) v = base[(size_t)(c + e) * p.col_stride];
-    else if (e == rem) v = MONT_ONE;
-    s[j] = v;
-  }
-  tip5_perm_pair(s, l, lut, rc);
-  if (active) {
-    const size_t per = p.nrows >> p.log_r;
-    const size_t coset = m / per, k = m - coset * per;
-    u64 *d = p.digests + (coset + (k << p.log_r)) * 5;
-    d[l] = s[0];
-    d[l + 2] = s[1];
-    if (l == 0) d[4] = s[2];
-  }
-}
-
-static constexpr int HASHQ_THREADS = 128;
-__global__ void __launch_bounds__(HASHQ_THREADS) tip5_hash_rows_quad_kernel(HashRowsParams p) {
-  __shared__ unsigned char lut[256];
-  __shared__ u64 rc[80];
-  for (int i = threadIdx.x; i < 256; i += blockDim.x) lut[i] = c_tip5_lut[i];
-  for (int i = threadIdx.x; i < 80; i += blockDim.x) rc[i] = c_tip5_rc[i];
-  __syncthreads();
-  const int lane = threadIdx.x & 31, l = lane & 3, group_base = lane & ~3;
-  size_t m = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 2;   // one row per 4 lanes
-  const bool active = m < p.nrows;
-  if (!active) m = p.nrows - 1;                                     // keep the quad alive for the shuffles
-  size_t per = p.nrows >> p.log_r;
-  size_t coset = m / per, k = m - coset * per;
-  size_t row = coset + (k << p.log_r);
-  const u64 *base = p.table + m;
-  u64 s[4] = {0, 0, 0, 0};
-  unsigned c = 0;
-  for (; c + 10 <= p.ncols; c += 10) {
-    s[0] = base[(size_t)(c + l) * p.col_stride];
-    s[1] = base[(size_t)(c + l + 4) * p.col_stride];
-    if (l < 2) s[2] = base[(size_t)(c + l + 8) * p.col_stride];
-    tip5_perm_quad(s, l, group_base, lut, rc);
-  }
-  unsigned rem = p.ncols - c;
-#pragma unroll
-  for (int i = 0; i < 3; i++) {
-    unsigned e = (unsigned)(l + 4 * i);
-    if (e < 10) {
-      u64 v = 0;
-      if (e < rem) v = base[(size_t)(c + e) * p.col_stride];
-      else if (e == rem) v = MONT_ONE;
-      s[i] = v;
-    }
-  }
-  tip5_perm_quad(s, l, group_base, lut, rc);
-  if (active) {
-    u64 *d = p.digests + row * 5;
-    d[l] = s[0];
-    if (l == 0) d[4] = s[1];
-  }
-}
-
 void hash_rows_run(Ctx &c, const u64 *table, size_t col_stride, size_t nrows, unsigned ncols, int log_r, u64 *digests,
                    unsigned coset_mem_stride) {
   HashRowsParams p{table, col_stride, nrows, ncols, log_r, digests, coset_mem_stride};
-  static const bool use_thread_per_row = getenv("TVM_TIP5_THREAD_PER_ROW") != nullptr;
-  static const bool use_imad_mds = getenv("TVM_TIP5_IMAD_MDS") != nullptr;   // A/B: the round-1 default (MDS on the integer pipe)
-  if (!use_imad_mds && !use_thread_per_row && !getenv("TVM_TIP5_ONE_ROW_PER_QUAD") && !getenv("TVM_TIP5_TWO_LANES") &&
-      !getenv("TVM_TIP5_SMEM_EXCHANGE")) {
-    const size_t rows_per_cta = HASHM_THREADS / 2;
-    unsigned grid = (unsigned)((nrows + rows_per_cta - 1) / rows_per_cta);
-    static const bool no_tma = getenv("TVM_TIP5_NO_TMA") != nullptr;        // A/B: per-lane LDG instead of bulk-copy staging
-    const size_t per = nrows >> log_r;
-    const bool tma_ok = !no_tma && nrows % rows_per_cta == 0 && per % rows_per_cta == 0 && ((uintptr_t)table % 16) == 0 &&
-                        (col_stride * sizeof(u64)) % 16 == 0;
-    if (tma_ok) tip5_hash_rows_mma_tma_kernel<<<grid, HASHM_THREADS, 0, c.stream>>>(p);
-    else tip5_hash_rows_mma_kernel<<<grid, HASHM_THREADS, 0, c.stream>>>(p);
-  } else if (coset_mem_stride != 1) {   // of the A/B variants only quad2 knows about strided cosets
-    const size_t rows_per_cta = HASHQ2_THREADS / 2;
-    unsigned grid = (unsigned)((nrows + rows_per_cta - 1) / rows_per_cta);
-    tip5_hash_rows_quad2_kernel<false><<<grid, HASHQ2_THREADS, 0, c.stream>>>(p);
-  } else if (use_thread_per_row) {
-    unsigned grid = (unsigned)((nrows + HASH_THREADS - 1) / HASH_THREADS);
-    tip5_hash_rows_kernel<<<grid, HASH_THREADS, 0, c.stream>>>(p);
-  } else if (getenv("TVM_TIP5_ONE_ROW_PER_QUAD")) {
-    size_t threads = nrows * 4;
-    unsigned grid = (unsigned)((threads + HASHQ_THREADS - 1) / HASHQ_THREADS);
-    tip5_hash_rows_quad_kernel<<<grid, HASHQ_THREADS, 0, c.stream>>>(p);
-  } else if (getenv("TVM_TIP5_TWO_LANES")) {   // A/B switch: measured 3 % slower than the default below at 2^20
-    unsigned grid = (unsigned)((nrows * 2 + HASHP_THREADS - 1) / HASHP_THREADS);
-    tip5_hash_rows_pair_kernel<<<grid, HASHP_THREADS, 0, c.stream>>>(p);
-  } else {
-    const size_t rows_per_cta = HASHQ2_THREADS / 2;
-    unsigned grid = (unsigned)((nrows + rows_per_cta - 1) / rows_per_cta);
-    // exchanging the MDS inputs through shared memory instead of shuffles measured 10 % SLOWER at 2^20 (191 vs 174 ms
-    // for the main table): kept as an A/B switch only
-    if (getenv("TVM_TIP5_SMEM_EXCHANGE")) tip5_hash_rows_quad2_kernel<true><<<grid, HASHQ2_THREADS, 0, c.stream>>>(p);
-    else tip5_hash_rows_quad2_kernel<false><<<grid, HASHQ2_THREADS, 0, c.stream>>>(p);
-  }
+  const size_t rows_per_cta = HASHM_THREADS / 2;
+  unsigned grid = (unsigned)((nrows + rows_per_cta - 1) / rows_per_cta);
+  const size_t per = nrows >> log_r;
+  const bool tma_ok = nrows % rows_per_cta == 0 && per % rows_per_cta == 0 && ((uintptr_t)table % 16) == 0 &&
+                      (col_stride * sizeof(u64)) % 16 == 0;
+  if (tma_ok) tip5_hash_rows_mma_tma_kernel<<<grid, HASHM_THREADS, 0, c.stream>>>(p);
+  else tip5_hash_rows_mma_kernel<<<grid, HASHM_THREADS, 0, c.stream>>>(p);
   c.launches++;
   TVM_CUDA(cudaGetLastError());
 }
 
-static void merkle_level_launch(Ctx &c, u64 *nodes, size_t lo, size_t count, bool thread_per_node) {
-  if (thread_per_node || count < 64) {
+static void merkle_level_launch(Ctx &c, u64 *nodes, size_t lo, size_t count) {
+  if (count < 64) {
     unsigned grid = (unsigned)((count + HASH_THREADS - 1) / HASH_THREADS);
     merkle_level_kernel<<<grid, HASH_THREADS, 0, c.stream>>>(nodes, lo, count);
   } else {
@@ -974,9 +555,8 @@ static void merkle_level_launch(Ctx &c, u64 *nodes, size_t lo, size_t count, boo
 void merkle_run(Ctx &c, u64 *nodes, size_t nleaves) {
   size_t w = nleaves / 2;
   const size_t TOP = 64;
-  static const bool thread_per_node = getenv("TVM_TIP5_IMAD_MDS") != nullptr;
   for (; w > TOP; w >>= 1) {
-    merkle_level_launch(c, nodes, w, w, thread_per_node);
+    merkle_level_launch(c, nodes, w, w);
   }
   if (w >= 1) {
     merkle_top_kernel<<<1, HASH_THREADS, 0, c.stream>>>(nodes, w);
@@ -992,8 +572,7 @@ void merkle_run_sharded(Ctx &c, u64 *nodes, size_t nleaves, unsigned rank, unsig
   if (W <= 1 || nleaves < 2 * (size_t)W) { merkle_run(c, nodes, nleaves); return; }
   for (size_t w = nleaves / 2; w >= W; w >>= 1) {
     const size_t cnt = w / W;
-    static const bool thread_per_node = getenv("TVM_TIP5_IMAD_MDS") != nullptr;
-    merkle_level_launch(c, nodes, w + rank * cnt, cnt, thread_per_node);
+    merkle_level_launch(c, nodes, w + rank * cnt, cnt);
   }
   TVM_CUDA(cudaGetLastError());
   c.all_gather(nodes + 5 * (size_t)W, 40);
