@@ -355,18 +355,42 @@ void tvm_execution_destroy(tvm_execution *ex);
  * point: `roots` m distinct canonical elements; a_out, b_out [m] canonical coefficients, lowest first. */
 int tvm_bezout_coefficients(tvm_ctx *ctx, const uint64_t *roots, uint64_t m, uint64_t *a_out, uint64_t *b_out);
 /* ---- STIR as a stand-alone low-degree test: Stir::prove / Stir::verify (low_degree_test/stir.rs:885-993, 995-1108) of the sealed
- *      `LowDegreeTest` trait (mod.rs:48-100) for ARBITRARY StirParameters (stir.rs:395-435; folding factor 2^2 as Stark::ldt fixes
- *      it, stark.rs:2023).  Used by the restated property tests of the reference (stir.rs:1813-2010) and by hosts that keep
- *      Prover::prove's orchestration.  The initial domain has 2^(log2_high_degree_bound + log2_initial_expansion_factor) points and
- *      offset BFieldElement::generator() (stir.rs:589).
- *      codeword   [len][3] canonical X-field evaluations on that domain (host or device memory)
+ *      `LowDegreeTest` trait (mod.rs:48-100) for ARBITRARY StirParameters (stir.rs:395-435), folding factor included.  Used by the
+ *      restated property tests of the reference (stir.rs:1813-2010) and by hosts that keep Prover::prove's orchestration and pick
+ *      their own low-degree test.  The initial domain has 2^(log2_high_degree_bound + log2_initial_expansion_factor) points and
+ *      offset BFieldElement::generator() (stir.rs:589); the folding factor is 2^log2_folding_factor.
+ *      Parameter errors are LdtParameterError's (stir.rs:437-459, 570-592), checked in the reference's order: TVM_ERR_LDT_PARAMS
+ *      for log2_folding_factor < 2 (TooSmallLog2FoldingFactor), log2_initial_expansion_factor == 0 (TooSmallInitialExpansionFactor),
+ *      log2_high_degree_bound < log2_folding_factor (TooLowDegreeOfHighDegreePolynomials), log2_folding_factor >= 64
+ *      (TooBigLog2FoldingFactor) or an initial domain beyond 2^32 points (InitialDomainTooBig); the variant is named in
+ *      tvm_last_error / `failure`.  Argument and parameter errors return before any kernel is launched. --- */
+typedef struct tvm_stir_info {
+  uint64_t domain_len, domain_offset, folding_factor;   /* initial domain (domain_offset canonical) and k = 2^log2_folding_factor */
+  uint64_t num_rounds;                                  /* full rounds */
+  uint64_t in_domain_queries[16], out_of_domain_queries[16];   /* per full round */
+  uint64_t final_num_queries, final_degree;             /* final round: in-domain queries, degree of the final polynomial */
+} tvm_stir_info;
+/* host code, no GPU: StirParameters::try_into_stir (stir.rs:437-567) */
+int tvm_stir_derive(uint32_t security_level, uint32_t soundness, uint32_t log2_folding_factor, uint32_t log2_initial_expansion_factor,
+                    uint32_t log2_high_degree_bound, tvm_stir_info *out);
+/*      codeword   [len][3] canonical X-field evaluations on the initial domain (host or device memory)
  *      proof_out  the encoded proof stream of the STIR items alone (Proof.0 layout; same capacity protocol as tvm_prove)
- *      indices_out (optional) receives the revealed first-round indices; *num_indices in: capacity, out: count. --- */
+ *      indices_out (optional) receives the revealed first-round indices; *num_indices in: capacity, out: count.
+ *      The device prover takes initial domains of up to 2^26 points (beyond: TVM_ERR_DOMAIN) and, on them, every folding factor
+ *      the derivation accepts (up to 2^25).  A response reveals at most 4096 distinct stacked leaves of 3 * 2^log2_folding_factor
+ *      words each; a round that would reveal more returns TVM_ERR_UNSUPPORTED before it writes any of them. */
+int tvm_stir_prove_k(tvm_ctx *ctx, uint32_t security_level, uint32_t soundness, uint32_t log2_folding_factor,
+                     uint32_t log2_initial_expansion_factor, uint32_t log2_high_degree_bound, const uint64_t *codeword, uint64_t *proof_out,
+                     size_t *proof_len, uint32_t *indices_out, size_t *num_indices);
+/* host code, no GPU; TVM_OK = accepted, TVM_ERR_VERIFICATION = rejected (`failure` names the LdtVerificationError variant);
+ * on acceptance the verifier's postscript: first-round indices and the partial first codeword [count][3] (optional outputs) */
+int tvm_stir_verify_k(uint32_t security_level, uint32_t soundness, uint32_t log2_folding_factor, uint32_t log2_initial_expansion_factor,
+                      uint32_t log2_high_degree_bound, const uint64_t *proof, size_t proof_len, uint32_t *indices_out, uint64_t *values_out,
+                      size_t *num_indices, char *failure, size_t failure_capacity);
+/* the two with log2_folding_factor = 2, the factor Stark::ldt uses (stark.rs:2023) */
 int tvm_stir_prove(tvm_ctx *ctx, uint32_t security_level, uint32_t soundness, uint32_t log2_initial_expansion_factor,
                    uint32_t log2_high_degree_bound, const uint64_t *codeword, uint64_t *proof_out, size_t *proof_len,
                    uint32_t *indices_out, size_t *num_indices);
-/* host code, no GPU; TVM_OK = accepted, TVM_ERR_VERIFICATION = rejected (`failure` names the LdtVerificationError variant);
- * on acceptance the verifier's postscript: first-round indices and the partial first codeword [count][3] (optional outputs) */
 int tvm_stir_verify(uint32_t security_level, uint32_t soundness, uint32_t log2_initial_expansion_factor, uint32_t log2_high_degree_bound,
                     const uint64_t *proof, size_t proof_len, uint32_t *indices_out, uint64_t *values_out, size_t *num_indices,
                     char *failure, size_t failure_capacity);

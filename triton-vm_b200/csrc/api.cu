@@ -911,16 +911,39 @@ int tvm_bezout_coefficients(tvm_ctx *ctx, const uint64_t *roots, uint64_t m, uin
   TVM_API_END
 }
 
-int tvm_stir_prove(tvm_ctx *ctx, uint32_t security_level, uint32_t soundness, uint32_t log2_initial_expansion_factor,
-                   uint32_t log2_high_degree_bound, const uint64_t *codeword, uint64_t *proof_out, size_t *proof_len,
-                   uint32_t *indices_out, size_t *num_indices) {
-  if (!ctx || !codeword || !proof_len || soundness > 1) return TVM_ERR_INVALID_ARG;
-  if (log2_high_degree_bound + log2_initial_expansion_factor > 26) return TVM_ERR_DOMAIN;
+int tvm_stir_derive(uint32_t security_level, uint32_t soundness, uint32_t log2_folding_factor, uint32_t log2_initial_expansion_factor,
+                    uint32_t log2_high_degree_bound, tvm_stir_info *out) {
+  if (!out || soundness > 1) return TVM_ERR_INVALID_ARG;
   StirDerived sd{};
-  if (int rc = stir_derive(security_level, STIR_LOG2_FOLDING_FACTOR, log2_initial_expansion_factor, log2_high_degree_bound, soundness == 1, sd))
+  if (int rc = stir_derive(security_level, log2_folding_factor, log2_initial_expansion_factor, log2_high_degree_bound, soundness == 1, sd))
     return rc;
+  *out = tvm_stir_info{};
+  out->domain_len = (uint64_t)1 << (log2_high_degree_bound + log2_initial_expansion_factor);
+  out->domain_offset = 7;                                   // BFieldElement::generator(), stir.rs:589
+  out->folding_factor = sd.folding_factor;
+  out->num_rounds = (uint64_t)sd.num_rounds;
+  for (int i = 0; i < sd.num_rounds; i++) {
+    out->in_domain_queries[i] = sd.in_domain[i];
+    out->out_of_domain_queries[i] = sd.out_of_domain[i];
+  }
+  out->final_num_queries = sd.final_num_in_domain_queries;
+  out->final_degree = sd.final_degree;
+  return TVM_OK;
+}
+
+int tvm_stir_prove_k(tvm_ctx *ctx, uint32_t security_level, uint32_t soundness, uint32_t log2_folding_factor,
+                     uint32_t log2_initial_expansion_factor, uint32_t log2_high_degree_bound, const uint64_t *codeword, uint64_t *proof_out,
+                     size_t *proof_len, uint32_t *indices_out, size_t *num_indices) {
+  if (!ctx || !codeword || !proof_len || soundness > 1) return TVM_ERR_INVALID_ARG;
   TVM_API_BEGIN(ctx)
   Ctx &c = *c__;
+  StirDerived sd{};
+  const char *why = "";
+  if (int rc = stir_derive(security_level, log2_folding_factor, log2_initial_expansion_factor, log2_high_degree_bound, soundness == 1, sd,
+                           &why))
+    throw ApiError{rc, why};
+  if (log2_high_degree_bound + log2_initial_expansion_factor > 26)
+    throw ApiError{TVM_ERR_DOMAIN, "STIR: the device prover supports initial domains of up to 2^26 points"};
   const size_t len = (size_t)1 << (log2_high_degree_bound + log2_initial_expansion_factor);
   std::vector<u64> proof;
   std::vector<uint32_t> revealed;
@@ -937,6 +960,15 @@ int tvm_stir_prove(tvm_ctx *ctx, uint32_t security_level, uint32_t soundness, ui
   copy_indices_out(revealed, indices_out, num_indices);
   copy_proof_out(proof, proof_out, proof_len);
   TVM_API_END
+}
+
+int tvm_stir_prove(tvm_ctx *ctx, uint32_t security_level, uint32_t soundness, uint32_t log2_initial_expansion_factor,
+                   uint32_t log2_high_degree_bound, const uint64_t *codeword, uint64_t *proof_out, size_t *proof_len,
+                   uint32_t *indices_out, size_t *num_indices) {
+  if (!ctx || !codeword || !proof_len || soundness > 1) return TVM_ERR_INVALID_ARG;
+  if (log2_high_degree_bound + log2_initial_expansion_factor > 26) return TVM_ERR_DOMAIN;
+  return tvm_stir_prove_k(ctx, security_level, soundness, STIR_LOG2_FOLDING_FACTOR, log2_initial_expansion_factor, log2_high_degree_bound,
+                          codeword, proof_out, proof_len, indices_out, num_indices);
 }
 
 int tvm_fri_derive(uint32_t security_level, uint32_t soundness, uint32_t log2_initial_expansion_factor, uint32_t log2_high_degree_bound,

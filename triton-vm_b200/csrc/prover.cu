@@ -86,8 +86,19 @@ size_t stir_num_ood_queries(unsigned security, unsigned log2_poly_degree, unsign
 }
 }  // namespace
 
-int stir_derive(unsigned security, unsigned log2_ff, unsigned log2_initial_exp, unsigned log2_hdb, bool conj, StirDerived &out) {
-  if (log2_ff < 2 || log2_initial_exp == 0 || log2_hdb < log2_ff || log2_hdb + log2_initial_exp > 32) return TVM_ERR_LDT_PARAMS;
+int stir_derive(unsigned security, unsigned log2_ff, unsigned log2_initial_exp, unsigned log2_hdb, bool conj, StirDerived &out,
+                const char **error) {
+  auto reject = [&](const char *what) {
+    if (error) *error = what;
+    return TVM_ERR_LDT_PARAMS;
+  };
+  // stir.rs:438-459, in the reference's order; a usize shift by 64 or more overflows
+  if (log2_ff < 2) return reject("LdtParameterError: TooSmallLog2FoldingFactor");
+  if (log2_initial_exp == 0) return reject("LdtParameterError: TooSmallInitialExpansionFactor");
+  if (log2_hdb < log2_ff) return reject("LdtParameterError: TooLowDegreeOfHighDegreePolynomials");
+  if (log2_ff >= 64) return reject("LdtParameterError: TooBigLog2FoldingFactor");
+  // StirParameters::initial_domain (stir.rs:570-592): ArithmeticDomain::of_length needs a 2-power root of unity of its order
+  if ((unsigned long long)log2_hdb + log2_initial_exp > 32) return reject("LdtParameterError: InitialDomainTooBig");
   out = StirDerived{};
   out.folding_factor = (size_t)1 << log2_ff;
   size_t folded_poly_degree = (((size_t)1 << log2_hdb) - 1) / out.folding_factor;
@@ -99,7 +110,7 @@ int stir_derive(unsigned security, unsigned log2_ff, unsigned log2_initial_exp, 
     size_t ood = stir_num_ood_queries(security, (unsigned)ilog2(folded_poly_degree), log2_next_exp, conj);
     size_t next_deg = folded_poly_degree / out.folding_factor;
     if (in_domain + ood > next_deg) break;
-    if (out.num_rounds >= STIR_MAX_ROUNDS) return TVM_ERR_LDT_PARAMS;
+    if (out.num_rounds >= STIR_MAX_ROUNDS) return reject("STIR: more than 16 full rounds");
     out.in_domain[out.num_rounds] = in_domain; out.out_of_domain[out.num_rounds] = ood; out.num_rounds++;
     folded_poly_degree = next_deg;
     log2_exp = log2_next_exp;

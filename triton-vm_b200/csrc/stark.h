@@ -43,8 +43,9 @@ struct StarkDerived {
 };
 // the Reed-Solomon code's proximity parameter δ of the regime (low_degree_test/mod.rs:243-320)
 double rs_proximity_parameter(unsigned log2_expansion, bool conjectured);
+// TVM_OK or TVM_ERR_LDT_PARAMS; `error` (optional) receives the name of the LdtParameterError variant
 int stir_derive(unsigned security_level, unsigned log2_folding_factor, unsigned log2_initial_expansion, unsigned log2_high_degree_bound,
-                bool conjectured, StirDerived &out);
+                bool conjectured, StirDerived &out, const char **error = nullptr);
 // TVM_OK or TVM_ERR_LDT_PARAMS; `error` (optional) receives the name of the LdtParameterError variant
 int fri_derive(unsigned security_level, bool conjectured, unsigned log2_initial_expansion, unsigned log2_high_degree_bound, FriDerived &out,
                const char **error = nullptr);

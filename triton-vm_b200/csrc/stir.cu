@@ -6,10 +6,12 @@
 //   poly' = (folded - Ans) / Zerofier * DegreeCorrection                 (stir.rs:950-966)
 // with dense polynomial arithmetic.  Here the same polynomial is obtained in evaluation form on
 // the next round's domain (whose points are disjoint from the quotient set: in-domain queries
-// live in offset^4<g^4>, the next domain is offset^3<g^2>, offset = 7^(3^t) is not in the 2-power
-// subgroup; out-of-domain queries are X-field elements) followed by one inverse NTT — exact field
-// arithmetic, hence the identical polynomial.  Ans and Zerofier (degree ~200) are interpolated on
-// the host and evaluated on the domain by zero-padded NTTs.
+// live in offset^k<g^k>, the next domain is offset^3<g^2>, offset = 7^(3^t), and offset^(k-3)
+// is outside the 2-power subgroup for every k < 2^30; out-of-domain queries are X-field elements)
+// followed by one inverse NTT — exact field arithmetic, hence the identical polynomial.  Ans and
+// Zerofier (degree ~200) are interpolated on the host and evaluated on the domain by zero-padded NTTs.
+// The folding factor k is any power of 2 from 4 on: k = 4 (Stark::ldt's) folds with one thread per
+// output, larger factors with one quad per output; a stacked leaf is 3k base-field words.
 //
 // Layout: X-field vectors are 3 planes; every buffer of a round is packed [3][len].
 #include <algorithm>
@@ -35,7 +37,7 @@ __global__ void stir_stack_kernel(const u64 *cw, size_t len, unsigned h, u64 *ou
   size_t lq = len / h, s = j / lq, i = j - s * lq;
   out[(3 * s + d) * lq + i] = cw[t];
 }
-// fold_polynomial: out_j = sum_{i<4} c_{4j+i} r^i   (stir.rs:1132-1147, folding factor 4)
+// fold_polynomial: out_j = sum_{i<4} c_{4j+i} r^i   (stir.rs:1132-1147, folding factor 4, the factor Stark::ldt uses)
 __global__ void stir_fold_kernel(const u64 *in, size_t in_len, xfe r1, xfe r2, xfe r3, u64 *out, size_t out_len) {
   size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= out_len) return;
@@ -47,6 +49,30 @@ __global__ void stir_fold_kernel(const u64 *in, size_t in_len, xfe r1, xfe r2, x
     if (k < in_len) acc = xadd(acc, xmul(xmake(in[k], in[in_len + k], in[2 * in_len + k]), rp[i]));
   }
   out[j] = acc.c0; out[out_len + j] = acc.c1; out[2 * out_len + j] = acc.c2;
+}
+// fold_polynomial for k = 2^log_k >= 8: out_j = sum_{i<k} c_{kj+i} r^i over in[3][k * out_len].  The four lanes of a quad
+// share one output: lane l reads the coefficients kj + l + 4m (m < k/4), so each load instruction of a warp reads eight whole
+// 32-byte sectors of a plane.  A lane folds its k/4 coefficients by Horner in r^4 and scales the sum by r^l; two butterfly
+// shuffles add up the quad.
+__global__ void stir_fold_quad_kernel(const u64 *in, size_t in_len, unsigned log_k, xfe r1, xfe r2, xfe r3, xfe r4, u64 *out,
+                                      size_t out_len) {
+  const size_t j = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 2;
+  const unsigned l = threadIdx.x & 3;
+  xfe h = xzero();
+  if (j < out_len) {            // no early return: every lane of the warp takes part in the shuffles
+    const size_t base = (j << log_k) + l;
+#pragma unroll 4
+    for (size_t m = (size_t)1 << (log_k - 2); m-- > 0;) {
+      const size_t i = base + 4 * m;
+      h = xadd(xmul(h, r4), xmake(in[i], in[in_len + i], in[2 * in_len + i]));
+    }
+    if (l) h = xmul(h, l == 1 ? r1 : l == 2 ? r2 : r3);
+  }
+#pragma unroll
+  for (int off = 1; off < 4; off <<= 1)
+    h = xadd(h, xmake(__shfl_xor_sync(0xffffffffu, h.c0, off), __shfl_xor_sync(0xffffffffu, h.c1, off),
+                      __shfl_xor_sync(0xffffffffu, h.c2, off)));
+  if (l == 0 && j < out_len) { out[j] = h.c0; out[out_len + j] = h.c1; out[2 * out_len + j] = h.c2; }
 }
 // out[d][j] = j < in_len ? in[d][j] * s^j : 0   for j < out_len  (coset pre-scaling + zero padding before an NTT)
 __global__ void stir_scale_pad_kernel(const u64 *in, size_t in_len, PowTab s, u64 *out, size_t out_len) {
@@ -169,7 +195,7 @@ XPoly xp_interpolate(const std::vector<xfe> &xs, const std::vector<xfe> &ys, con
   return out;
 }
 
-struct Commitment {        // StirMerkleTree: stacked leaves as a [12][leaves] column table + the node array
+struct Commitment {        // StirMerkleTree: stacked leaves as a [3k][leaves] column table + the node array
   u64 *stack = nullptr, *nodes = nullptr;
   size_t leaves = 0;
 };
@@ -179,8 +205,21 @@ struct Commitment {        // StirMerkleTree: stacked leaves as a [12][leaves] c
 std::vector<uint32_t> stir_prove_run(Ctx &c, DevMem &mem, ProofStream &ps, const u64 *d_codeword, size_t len, u64 offset_mont,
                                      const StirDerived &sd, u64 *d_tmp) {
   const unsigned ff = (unsigned)sd.folding_factor;
-  if (ff != 4) throw ApiError{TVM_ERR_UNSUPPORTED, "STIR: folding factor must be 4"};
+  const unsigned log_ff = (unsigned)ilog2s(ff);
+  if (ff < 4 || ff != 1u << log_ff || len % ff)
+    throw ApiError{TVM_ERR_UNSUPPORTED, "STIR: the folding factor must be a power of 2, at least 4, dividing the domain length"};
   auto launch_check = [&](int k) { c.launches += k; TVM_CUDA(cudaGetLastError()); };
+  // fold_polynomial (stir.rs:1132-1147) of d_in[3][k * out_len]
+  auto fold = [&](const u64 *d_in, size_t in_len, xfe r, u64 *d_out, size_t out_len) {
+    const xfe r2 = xmul(r, r), r3 = xmul(r2, r);
+    if (ff == 4) {
+      stir_fold_kernel<<<st_grid(out_len), ST_THREADS, 0, c.stream>>>(d_in, in_len, r, r2, r3, d_out, out_len);
+    } else {
+      stir_fold_quad_kernel<<<st_grid(4 * out_len), ST_THREADS, 0, c.stream>>>(d_in, in_len, log_ff, r, r2, r3, xmul(r2, r2), d_out,
+                                                                               out_len);
+    }
+    launch_check(1);
+  };
 
   auto commit = [&](const u64 *d_cw, size_t L) {
     Commitment cm;
@@ -219,11 +258,13 @@ std::vector<uint32_t> stir_prove_run(Ctx &c, DevMem &mem, ProofStream &ps, const
   constexpr size_t MAXQ = 4096, MAXN = MAXQ * 40;      // queries per round / authentication-structure nodes
   unsigned *d_idx = (unsigned *)mem.words(MAXQ);
   unsigned *d_nidx = (unsigned *)mem.words(MAXN);
-  u64 *d_gather = mem.words(MAXQ * 12);
+  // one response's leaves: no more distinct folded indices than leaves of the first (largest) tree, each of 3 * ff words
+  const size_t max_leaves = std::min(MAXQ, len / ff);
+  u64 *d_gather = mem.words(max_leaves * 3 * ff);
   u64 *d_dig = mem.words(MAXN * 5);
   // StirResponse {queried_leafs, auth_structure} of a commitment at the (folded, de-duplicated) indices
   auto respond = [&](const Commitment &cm, const std::vector<uint32_t> &idx) {
-    if (idx.size() > MAXQ) throw ApiError{TVM_ERR_UNSUPPORTED, "STIR: too many queries"};
+    if (idx.size() > max_leaves) throw ApiError{TVM_ERR_UNSUPPORTED, "STIR: more than 4096 distinct queried leaves in one round"};
     TVM_CUDA(cudaMemcpyAsync(d_idx, idx.data(), idx.size() * 4, cudaMemcpyHostToDevice, c.stream));
     gather_rows_run(c, cm.stack, cm.leaves, 3 * ff, d_idx, (unsigned)idx.size(), 0, -1, d_gather);
     std::vector<u64> rows = d2h(c, d_gather, idx.size() * 3 * ff);
@@ -282,10 +323,9 @@ std::vector<uint32_t> stir_prove_run(Ctx &c, DevMem &mem, ProofStream &ps, const
     const xfe r = ps.sample_scalars(1)[0];
     const size_t f_len = cur_len / ff, n_len = cur_len / 2;
     const u64 n_off = fmul(fmul(cur_off, cur_off), cur_off);                 // next_round_domain: offset^2 * offset
-    const u64 f_off = fmul(fmul(cur_off, cur_off), fmul(cur_off, cur_off));  // domain.pow(4)
+    const u64 f_off = fpow(cur_off, ff);                                      // domain.pow(folding_factor)
     u64 *d_folded = mem.words(3 * f_len);
-    stir_fold_kernel<<<st_grid(f_len), ST_THREADS, 0, c.stream>>>(d_poly, cur_len, r, xmul(r, r), xmul(xmul(r, r), r), d_folded, f_len);
-    launch_check(1);
+    fold(d_poly, cur_len, r, d_folded, f_len);
     u64 *d_scratch = mem.words(3 * n_len);
     u64 *d_fe = mem.words(3 * n_len);          // folded evaluations on the next round's domain
     evaluate(d_folded, f_len, n_off, n_len, d_fe, d_scratch);
@@ -319,7 +359,7 @@ std::vector<uint32_t> stir_prove_run(Ctx &c, DevMem &mem, ProofStream &ps, const
     // answers of the folded polynomial at the queried points of the folded domain (stir.rs:942-957)
     std::vector<xfe> points, answers;
     {
-      u64 *d_ff = d_scratch;                  // folded polynomial on offset^4 <g^4>, [3][f_len]
+      u64 *d_ff = d_scratch;                  // folded polynomial on offset^k <g^k>, [3][f_len]
       u64 *d_ff_in = mem.words(3 * f_len);
       evaluate(d_folded, f_len, f_off, f_len, d_ff, d_ff_in);
       mem.release(d_ff_in);
@@ -394,8 +434,7 @@ std::vector<uint32_t> stir_prove_run(Ctx &c, DevMem &mem, ProofStream &ps, const
     const xfe r = ps.sample_scalars(1)[0];
     const size_t f_len = cur_len / ff;
     u64 *d_final = mem.words(3 * f_len);
-    stir_fold_kernel<<<st_grid(f_len), ST_THREADS, 0, c.stream>>>(d_poly, cur_len, r, xmul(r, r), xmul(xmul(r, r), r), d_final, f_len);
-    launch_check(1);
+    fold(d_poly, cur_len, r, d_final, f_len);
     std::vector<u64> co = d2h(c, d_final, 3 * f_len);
     size_t deg_plus_1 = f_len;
     while (deg_plus_1 > 0 && co[deg_plus_1 - 1] == 0 && co[f_len + deg_plus_1 - 1] == 0 && co[2 * f_len + deg_plus_1 - 1] == 0) deg_plus_1--;

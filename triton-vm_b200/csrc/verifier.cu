@@ -717,16 +717,20 @@ LdtResult stir_verify(Transcript &ps, const StarkDerived &d) {
 }  // namespace tvm
 
 // Stir::verify as a stand-alone low-degree test (stir.rs:995-1108) for arbitrary StirParameters
-extern "C" int tvm_stir_verify(uint32_t security_level, uint32_t soundness, uint32_t log2_initial_expansion_factor,
-                               uint32_t log2_high_degree_bound, const uint64_t *proof, size_t proof_len, uint32_t *indices_out,
-                               uint64_t *values_out, size_t *num_indices, char *failure, size_t failure_capacity) {
+extern "C" int tvm_stir_verify_k(uint32_t security_level, uint32_t soundness, uint32_t log2_folding_factor,
+                                 uint32_t log2_initial_expansion_factor, uint32_t log2_high_degree_bound, const uint64_t *proof,
+                                 size_t proof_len, uint32_t *indices_out, uint64_t *values_out, size_t *num_indices, char *failure,
+                                 size_t failure_capacity) {
   using namespace tvm;
   set_failure(failure, failure_capacity, "");
   if (!proof || !proof_len || soundness > 1) return TVM_ERR_INVALID_ARG;
   StarkDerived d{};
-  if (int rc = stir_derive(security_level, STIR_LOG2_FOLDING_FACTOR, log2_initial_expansion_factor, log2_high_degree_bound, soundness == 1,
-                           d.stir))
+  const char *why = "";
+  if (int rc = stir_derive(security_level, log2_folding_factor, log2_initial_expansion_factor, log2_high_degree_bound, soundness == 1, d.stir,
+                           &why)) {
+    set_failure(failure, failure_capacity, why);
     return rc;
+  }
   d.ldt = 2;
   d.ldt_len = (size_t)1 << (log2_high_degree_bound + log2_initial_expansion_factor);
   d.ldt_offset = 7;                                   // BFieldElement::generator(), stir.rs:589
@@ -754,6 +758,13 @@ extern "C" int tvm_stir_verify(uint32_t security_level, uint32_t soundness, uint
     set_failure(failure, failure_capacity, "internal error");
     return TVM_ERR_VERIFICATION;
   }
+}
+
+extern "C" int tvm_stir_verify(uint32_t security_level, uint32_t soundness, uint32_t log2_initial_expansion_factor,
+                               uint32_t log2_high_degree_bound, const uint64_t *proof, size_t proof_len, uint32_t *indices_out,
+                               uint64_t *values_out, size_t *num_indices, char *failure, size_t failure_capacity) {
+  return tvm_stir_verify_k(security_level, soundness, tvm::STIR_LOG2_FOLDING_FACTOR, log2_initial_expansion_factor, log2_high_degree_bound,
+                           proof, proof_len, indices_out, values_out, num_indices, failure, failure_capacity);
 }
 
 // Fri::verify as a stand-alone low-degree test (fri.rs:774-789) for arbitrary FriParameters: the fri_verify of tvm_verify

@@ -66,6 +66,12 @@ class FriInfo(ctypes.Structure):   # tvm_fri_info
         "domain_len", "domain_offset", "expansion_factor", "max_degree", "num_collinearity_checks", "num_rounds", "last_round_max_degree")]
 
 
+class StirInfo(ctypes.Structure):   # tvm_stir_info
+    _fields_ = [(n, ctypes.c_uint64) for n in ("domain_len", "domain_offset", "folding_factor", "num_rounds")] + [
+        ("in_domain_queries", ctypes.c_uint64 * 16), ("out_of_domain_queries", ctypes.c_uint64 * 16),
+        ("final_num_queries", ctypes.c_uint64), ("final_degree", ctypes.c_uint64)]
+
+
 class ClaimStruct(ctypes.Structure):
     _fields_ = [("program_digest", ctypes.c_uint64 * 5), ("version", ctypes.c_uint32), ("input", _u64p),
                 ("num_input", ctypes.c_size_t), ("output", _u64p), ("num_output", ctypes.c_size_t)]
@@ -209,6 +215,11 @@ _SIGNATURES = {
                                       ctypes.POINTER(ctypes.c_size_t), ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_size_t)]),
     "tvm_stir_verify": (ctypes.c_int, [ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, _u64p, ctypes.c_size_t,
                                        ctypes.POINTER(ctypes.c_uint32), _u64p, ctypes.POINTER(ctypes.c_size_t), ctypes.c_char_p, ctypes.c_size_t]),
+    "tvm_stir_derive": (ctypes.c_int, [ctypes.c_uint32] * 5 + [ctypes.POINTER(StirInfo)]),
+    "tvm_stir_prove_k": (ctypes.c_int, [_vp] + [ctypes.c_uint32] * 5 + [_u64p, _u64p, ctypes.POINTER(ctypes.c_size_t),
+                                        ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_size_t)]),
+    "tvm_stir_verify_k": (ctypes.c_int, [ctypes.c_uint32] * 5 + [_u64p, ctypes.c_size_t, ctypes.POINTER(ctypes.c_uint32), _u64p,
+                                         ctypes.POINTER(ctypes.c_size_t), ctypes.c_char_p, ctypes.c_size_t]),
     "tvm_fri_derive": (ctypes.c_int, [ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, ctypes.POINTER(FriInfo)]),
     "tvm_fri_prove": (ctypes.c_int, [_vp, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, _u64p, ctypes.c_size_t, _u64p,
                                      ctypes.POINTER(ctypes.c_size_t), ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_size_t)]),
@@ -255,15 +266,16 @@ def lib():
     return _lib
 
 
-def _ldt_verify(entry, cap, security_level, log2_expansion, log2_high_degree_bound, proof, conjectured):
-    """a stand-alone low-degree test's verifier (tvm_stir_verify / tvm_fri_verify) with room for `cap` revealed indices"""
+def _ldt_verify(entry, cap, security_level, log2_expansion, log2_high_degree_bound, proof, conjectured, *extra):
+    """a stand-alone low-degree test's verifier (tvm_stir_verify_k / tvm_fri_verify) with room for `cap` revealed indices;
+    `extra` are the arguments between the soundness and log2_expansion (tvm_stir_verify_k's log2_folding_factor)"""
     pr, prp = _np_u64(proof)
     icap = ctypes.c_size_t(cap)
     idx = (ctypes.c_uint32 * cap)()
     vals = np.zeros((cap, 3), dtype=np.uint64)
     msg = ctypes.create_string_buffer(256)
-    rc = entry(security_level, int(conjectured), log2_expansion, log2_high_degree_bound, prp, pr.size, idx, vals.ctypes.data_as(_u64p),
-               ctypes.byref(icap), msg, 256)
+    rc = entry(security_level, int(conjectured), *extra, log2_expansion, log2_high_degree_bound, prp, pr.size, idx,
+               vals.ctypes.data_as(_u64p), ctypes.byref(icap), msg, 256)
     if rc == 0:
         k = icap.value
         return True, "", [int(idx[i]) for i in range(k)], vals[:k].copy()
@@ -272,9 +284,24 @@ def _ldt_verify(entry, cap, security_level, log2_expansion, log2_high_degree_bou
     _check_plain(rc, msg.value.decode())
 
 
-def stir_verify(security_level, log2_expansion, log2_high_degree_bound, proof, conjectured=False):
-    """Stir::verify for arbitrary StirParameters (host code, no GPU) -> (accepted, failure, first-round indices, partial first codeword [k,3])"""
-    return _ldt_verify(lib().tvm_stir_verify, 8192, security_level, log2_expansion, log2_high_degree_bound, proof, conjectured)
+def stir_verify(security_level, log2_expansion, log2_high_degree_bound, proof, conjectured=False, log2_folding_factor=2):
+    """Stir::verify for arbitrary StirParameters (host code, no GPU) -> (accepted, failure, first-round indices, partial first
+    codeword [k,3]).  Parameter errors raise TvmError (TVM_ERR_LDT_PARAMS = -6, the LdtParameterError variant in the message)."""
+    return _ldt_verify(lib().tvm_stir_verify_k, 8192, security_level, log2_expansion, log2_high_degree_bound, proof, conjectured,
+                       log2_folding_factor)
+
+
+def stir_derive(security_level, log2_expansion, log2_high_degree_bound, conjectured=False, log2_folding_factor=2):
+    """StirParameters::try_into_stir (host code, no GPU) -> dict with the keys and values of oracle.stir.derive; raises TvmError
+    (TVM_ERR_LDT_PARAMS = -6) for parameters the reference rejects"""
+    out = StirInfo()
+    _check_plain(lib().tvm_stir_derive(security_level, int(conjectured), log2_folding_factor, log2_expansion, log2_high_degree_bound,
+                                       ctypes.byref(out)))
+    k = out.num_rounds
+    rounds = [(int(a), int(b)) for a, b in zip(out.in_domain_queries[:k], out.out_of_domain_queries[:k])]
+    return dict(initial_domain_len=int(out.domain_len), initial_offset=int(out.domain_offset), folding_factor=int(out.folding_factor),
+                round_queries=rounds, final_num_in_domain_queries=int(out.final_num_queries), final_degree=int(out.final_degree),
+                num_first_round_queries=rounds[0][0] if rounds else int(out.final_num_queries))
 
 
 def fri_derive(security_level, log2_expansion, log2_high_degree_bound, conjectured=False):
@@ -918,8 +945,9 @@ class Backend:
             self._h, ctypes.byref(p), ctypes.byref(cs), ph, mtp, int(bool(fill_derived_main_columns)), self._seed(seed), proof_out,
             proof_len), dom)
 
-    def stir_prove(self, security_level, log2_expansion, log2_high_degree_bound, codeword, conjectured=False):
-        """Stir::prove on the device for arbitrary StirParameters: codeword [2^(hdb+exp), 3] canonical -> (proof words, revealed indices)"""
+    def stir_prove(self, security_level, log2_expansion, log2_high_degree_bound, codeword, conjectured=False, log2_folding_factor=2):
+        """Stir::prove on the device for arbitrary StirParameters: codeword [2^(hdb+exp), 3] canonical (numpy, or a contiguous torch
+        tensor on the host or the device) -> (proof words, revealed indices)"""
         cw, cwp, shape = _u64_arg(codeword)
         n = 1 << (log2_high_degree_bound + log2_expansion)
         assert int(np.prod(shape)) == 3 * n
@@ -929,8 +957,9 @@ class Backend:
         est = 1 << 22
         buf = np.empty(est, dtype=np.uint64)
         cap.value = est
-        self._chk(self._l.tvm_stir_prove(self._h, security_level, int(conjectured), log2_expansion, log2_high_degree_bound, cwp,
-                                         buf.ctypes.data_as(_u64p), ctypes.byref(cap), idx, ctypes.byref(icap)))
+        self._chk(self._l.tvm_stir_prove_k(self._h, security_level, int(conjectured), log2_folding_factor, log2_expansion,
+                                           log2_high_degree_bound, cwp, buf.ctypes.data_as(_u64p), ctypes.byref(cap), idx,
+                                           ctypes.byref(icap)))
         return buf[:cap.value].copy(), [int(idx[i]) for i in range(icap.value)]
 
     def fri_prove(self, security_level, log2_expansion, log2_high_degree_bound, codeword, conjectured=False):
